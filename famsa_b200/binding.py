@@ -12,13 +12,15 @@ EXPORTED_SYMBOLS = [
     "famsa_abi_version", "famsa_create", "famsa_destroy", "famsa_last_error", "famsa_kernel_launches",
     "famsa_lcs_upload", "famsa_lcs_upload_sorted", "famsa_lcs_sorted_order", "famsa_lcs_last_tiles", "famsa_lcs_n_seqs", "famsa_lcs_triangle", "famsa_lcs_triangle_device",
     "famsa_device_alloc", "famsa_device_free", "famsa_ipc_export", "famsa_ipc_open", "famsa_ipc_close", "famsa_lcs_triangle_exchange",
-    "famsa_lcs_rows", "famsa_lcs_rows_device", "famsa_lcs_assign", "famsa_lcs_assign_shard", "famsa_lcs_upgma", "famsa_lcs_upgma_from_triangle", "famsa_lcs_prim", "famsa_transform_f64", "famsa_transform_f32",
+    "famsa_lcs_rows", "famsa_lcs_rows_device", "famsa_lcs_assign", "famsa_lcs_assign_shard", "famsa_lcs_upgma", "famsa_lcs_upgma_from_triangle", "famsa_lcs_prim", "famsa_dist_export", "famsa_transform_f64", "famsa_transform_f32",
     "famsa_lcs_last_timing", "famsa_dp_align_batch", "famsa_dp_align_batch_device", "famsa_dp_last_timing",
     "famsa_prof_set_scoring", "famsa_prof_put", "famsa_prof_merge_batch", "famsa_prof_get", "famsa_prof_drop",
     "famsa_prof_last_timing", "famsa_prof_stats", "famsa_prof_align_tree", "famsa_prof_tree_paths",
 ]
 
 PROF_LEAF = 0x80000000            # FAMSA_PROF_LEAF
+
+WRITE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_uint64)   # famsa_write_fn
 
 
 class DpProfile(C.Structure):
@@ -96,6 +98,8 @@ def load_library() -> C.CDLL:
     lib.famsa_lcs_upgma.argtypes = [vp, i32, i32, vp]
     lib.famsa_lcs_upgma_from_triangle.argtypes = [vp, i32, i32, vp, i32, vp]
     lib.famsa_lcs_assign_shard.argtypes = [vp, vp, u32, i32, u32, u32, vp, vp]
+    lib.famsa_dist_export.argtypes = [vp, i32, i32, i32, vp, vp, u64, WRITE_FN, vp, C.POINTER(u64)]
+    lib.famsa_debug_format_f32.argtypes = [vp, u64, vp, C.POINTER(u64)]
     lib.famsa_transform_f64.argtypes = [i32, u32, u32, u32]
     lib.famsa_transform_f64.restype = C.c_double
     lib.famsa_transform_f32.argtypes = [i32, u32, u32, u32]
@@ -234,6 +238,50 @@ class Engine:
         self._check(self.lib.famsa_lcs_rows(self.h, _ptr(ref), len(ref), _ptr(cols), n_col, _ptr(buf),
                                             buf.dtype.itemsize))
         return buf[:len(ref) * n_col].reshape(len(ref), n_col)
+
+    def dist_export(self, ids, kind: int = 0, square: bool = False, pid: bool = False, out=None,
+                    chunk_bytes: int = 0):
+        """famsa_dist_export: the -dist_export CSV of the set of the last upload() (caller order), byte for byte what
+        DistanceCalculator writes.  ids: the FASTA headers without '>' (str or bytes).  Returns the text as bytes, or,
+        with `out` (a binary file object), writes it there chunk by chunk and returns the byte count."""
+        raw = [i.encode() if isinstance(i, str) else bytes(i) for i in ids]
+        if len(raw) != self.n:
+            raise ValueError(f"{len(raw)} ids for {self.n} uploaded sequences")
+        blob = b"".join(raw)
+        offs = np.zeros(len(raw) + 1, dtype=np.uint64)
+        offs[1:] = np.cumsum([len(r) for r in raw], dtype=np.uint64)
+        buf = C.create_string_buffer(blob, max(len(blob), 1))
+        parts = bytearray() if out is None else None
+        failure = []
+
+        def sink(_user, ptr, n):
+            try:
+                view = memoryview((C.c_char * n).from_address(ptr)).cast("B")
+                if parts is None:
+                    out.write(view)
+                else:
+                    parts.extend(view)
+                return 0
+            except BaseException as e:          # reported after the call; the library stops writing
+                failure.append(e)
+                return 1
+
+        cb = WRITE_FN(sink)
+        written = C.c_uint64()
+        rc = self.lib.famsa_dist_export(self.h, kind, int(square), int(pid), buf, _ptr(offs), chunk_bytes, cb, None,
+                                        C.byref(written))
+        if failure:
+            raise failure[0]
+        self._check(rc)
+        return bytes(parts) if out is None else written.value
+
+    def debug_format_f32(self, values) -> bytes:
+        """famsa_debug_format_f32: the device formatter alone, every value followed by ','."""
+        v = np.ascontiguousarray(values, dtype=np.float32)
+        out = np.empty(max(40 * v.size, 1), dtype=np.uint8)
+        n = C.c_uint64()
+        self._check(self.lib.famsa_debug_format_f32(_ptr(v), v.size, _ptr(out), C.byref(n)))
+        return out[:n.value].tobytes()
 
     def prim(self, kind: int = 0):
         """MSTPrim's vertex loop on the device: (edge_from, edge_to, edge_dist, prim_order)."""

@@ -100,6 +100,7 @@ void famsa_destroy(famsa_ctx* ctx)
                           &S.d_assign, &S.d_mind, &S.d_tiles,
                           &S.d_res, &S.d_refpos, &S.d_ids_a, &S.d_ids_b, &S.d_out_stage, &S.d_masks64, &S.d_x64})
         b->release();
+    fb::dist_export_release(ctx);
     fb::prof_release_all(ctx);
     fb::DpState& D = ctx->dp;
     if (D.h_pinned) cudaFreeHost(D.h_pinned);
@@ -572,6 +573,31 @@ int famsa_lcs_assign_shard(famsa_ctx* ctx, const uint32_t* seed_ids, uint32_t n_
     if (!stream) { FB_CUDA(cudaStreamSynchronize(st)); fb::scratch_release(ctx, st, true); return finish_timing(ctx); }
     // the seed ids were handed to an async copy from pageable memory: staged by the driver before the call returned
     return fb::scratch_release(ctx, st, false);
+}
+
+int famsa_dist_export(famsa_ctx* ctx, int distance_kind, int square, int pid, const char* ids, const uint64_t* id_offsets,
+                      uint64_t chunk_bytes, famsa_write_fn write, void* user, uint64_t* bytes_written)
+{
+    FB_CHECK_CTX(ctx);
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (bytes_written) *bytes_written = 0;
+    if (ctx->lcs.n == 0) { set_error("famsa_dist_export: famsa_lcs_upload has not been called"); return FAMSA_E_STATE; }
+    if (!ctx->lcs.h_order.empty()) {
+        set_error("famsa_dist_export: the set was uploaded with famsa_lcs_upload_sorted; the export works in the caller's order "
+                  "(upload it with famsa_lcs_upload)");
+        return FAMSA_E_STATE;
+    }
+    if (!pid && distance_kind != 0 && distance_kind != 1) { set_error("famsa_dist_export: distance_kind must be 0 or 1"); return FAMSA_E_INVALID; }
+    if (!ids || !id_offsets || !write) { set_error("famsa_dist_export: NULL ids, id_offsets or write"); return FAMSA_E_INVALID; }
+    for (uint32_t i = 0; i < ctx->lcs.n; ++i)
+        if (id_offsets[i + 1] < id_offsets[i]) { set_error("famsa_dist_export: id_offsets must not decrease"); return FAMSA_E_INVALID; }
+    FB_CUDA(cudaSetDevice(ctx->device));
+    int rc = fb::scratch_acquire(ctx, ctx->stream);
+    if (rc) return rc;
+    rc = fb::dist_export(ctx, distance_kind, square, pid, ids, id_offsets, chunk_bytes, write, user, bytes_written);
+    cudaStreamSynchronize(ctx->stream);
+    fb::scratch_release(ctx, ctx->stream, true);
+    return rc;
 }
 
 int famsa_lcs_last_timing(const famsa_ctx* ctx, float* total_ms, float* main_kernel_ms, uint64_t* n_pairs)

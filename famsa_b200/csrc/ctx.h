@@ -58,6 +58,11 @@ struct LcsState {
         d_prim_dtri, d_prim_comp, d_prim_best, d_prim_part;
     // per-call scratch
     DevBuf d_tiles, d_res, d_refpos, d_ids_a, d_ids_b, d_out_stage, d_masks64, d_x64;
+    // famsa_dist_export: per-sequence tables, the two device text chunks and their pinned host twins
+    DevBuf d_dx_meta, d_dx_ids, d_dx_side, d_dx_colq, d_dx_chunk[2];
+    char* h_dx_chunk[2] = {nullptr, nullptr};
+    size_t h_dx_chunk_cap = 0;
+    cudaEvent_t ev_dx[6] = {};               // per chunk buffer: format start, format end, copy done
     // last-call timing
     float last_total_ms = 0.f, last_main_ms = 0.f;
     uint64_t last_pairs = 0;
@@ -224,6 +229,13 @@ int lcs_assign_shard(famsa_ctx* ctx, const uint32_t* h_seed_ids, uint32_t n_seed
 int lcs_prim(famsa_ctx* ctx, int kind, int32_t* h_from, int32_t* h_to, double* h_dist, int32_t* h_order);
 int lcs_assign(famsa_ctx* ctx, const uint32_t* h_seed_ids, uint32_t n_seeds, int kind, uint32_t* h_assign,
                float* h_mind);
+int lcs_pow075_f64(famsa_ctx* ctx, cudaStream_t st);
+int lcs_exact_block(famsa_ctx* ctx, const std::vector<uint32_t>& rows, const uint32_t* d_col_ids, uint32_t n_col, void* d_out,
+                    int elem_bytes, cudaStream_t st);
+// dist_export.cu
+int dist_export(famsa_ctx* ctx, int kind, int square, int pid, const char* ids, const uint64_t* id_offsets,
+                uint64_t chunk_bytes, famsa_write_fn write, void* user, uint64_t* bytes_written);
+void dist_export_release(famsa_ctx* ctx);
 // dp.cu
 int dp_run_host(famsa_ctx* ctx, const famsa_dp_job* jobs, uint32_t n, const int64_t gaps[4], famsa_dp_result* results,
                 uint8_t* path_buf, uint8_t* dirs_buf);

@@ -33,6 +33,7 @@
 #include <cooperative_groups.h>
 
 #include "ctx.h"
+#include "transform_dev.cuh"
 
 namespace fb {
 
@@ -457,17 +458,7 @@ __global__ void __launch_bounds__(128) k_lcs_exact_batch(const uint8_t* __restri
 // medoid assignment: float Transform + running arg-min over the seed rows (FastTree.cpp:309-324)
 // ------------------------------------------------------------------------------------------------
 
-// Transform<float, Distance> (AbstractTreeGenerator.hpp:28-82) with the host-computed (float) pow(i, 0.75) table;
-// IEEE division, so the result is the host's bit for bit.
-__device__ __forceinline__ float transform_f32(int kind, uint32_t lcs, uint32_t len1, uint32_t len2,
-                                               const float* __restrict__ pow075, float never)
-{
-    if (kind == 2) return __fdiv_rn((float)lcs, (float)(len1 < len2 ? len1 : len2));
-    const uint32_t indel_i = len1 + len2 - 2 * lcs;
-    if (!lcs) return never;                                  // (float) nextafter((double) FLT_MAX, 0) == FLT_MAX
-    if (kind == 0) return __fdiv_rn(pow075[indel_i], (float)lcs);
-    return __fdiv_rn((float)indel_i, (float)lcs);
-}
+// transform_f32 / transform_f64 (Transform<float|double, Distance>): transform_dev.cuh
 
 __global__ void k_assign(const void* __restrict__ lcs, int elem_bytes, uint32_t n, uint32_t n_seeds,
                          const uint32_t* __restrict__ seed_ids, const uint32_t* __restrict__ lens,
@@ -518,15 +509,6 @@ __global__ void k_assign_packed(const void* __restrict__ lcs, int elem_bytes, ui
 // ------------------------------------------------------------------------------------------------
 // MST-Prim vertex loop (MSTPrim<>::run_view, MSTPrim.cpp:280-549) on the resident LCS triangle
 // ------------------------------------------------------------------------------------------------
-
-__device__ __forceinline__ double transform_f64(int kind, uint32_t lcs, uint32_t len1, uint32_t len2,
-                                                const double* __restrict__ pow075, double never)
-{
-    const uint32_t indel_i = len1 + len2 - 2 * lcs;
-    if (!lcs) return never;                                  // nextafter(DBL_MAX, 0)
-    if (kind == 0) return __ddiv_rn(pow075[indel_i], (double)lcs);
-    return __ddiv_rn((double)indel_i, (double)lcs);
-}
 
 struct PrimState {                 // per sequence: best known connection to the tree
     double dist;
@@ -1463,6 +1445,30 @@ static int prim_boruvka(famsa_ctx* ctx, int kind, int eb, int32_t* h_from, int32
     return FAMSA_OK;
 }
 
+// (double) pow(i, 0.75) for every possible indel count into d_pow075_f64, host libm, like Transform<double,
+// indel075_div_lcs>'s table
+int lcs_pow075_f64(famsa_ctx* ctx, cudaStream_t st)
+{
+    LcsState& S = ctx->lcs;
+    std::vector<double> pw((size_t)2 * S.max_len + 2);
+    for (size_t v = 0; v < pw.size(); ++v) pw[v] = pow((double)v, 0.75);
+    FB_TRY(S.d_pow075_f64.reserve(sizeof(double) * pw.size()));
+    FB_CUDA(cudaMemcpyAsync(S.d_pow075_f64.p, pw.data(), sizeof(double) * pw.size(), cudaMemcpyHostToDevice, st));
+    FB_CUDA(cudaStreamSynchronize(st));          // pw goes out of scope
+    return FAMSA_OK;
+}
+
+// out[k * n_col + i] = LCS with sequence rows[k] as the row (seq0) against col_ids[i], by the reference recurrence for
+// every pair (k_lcs_exact_batch / k_lcs_exact): orientation-exact whatever the two sequences are
+int lcs_exact_block(famsa_ctx* ctx, const std::vector<uint32_t>& rows, const uint32_t* d_col_ids, uint32_t n_col, void* d_out,
+                    int elem_bytes, cudaStream_t st)
+{
+    std::vector<ExactReq> reqs;
+    reqs.reserve(rows.size());
+    for (size_t k = 0; k < rows.size(); ++k) reqs.push_back(ExactReq{rows[k], n_col, 0, k * n_col});
+    return exact_rows(ctx, reqs, d_col_ids, d_out, elem_bytes, st);
+}
+
 int lcs_prim(famsa_ctx* ctx, int kind, int32_t* h_from, int32_t* h_to, double* h_dist, int32_t* h_order)
 {
     LcsState& S = ctx->lcs;
@@ -1485,13 +1491,7 @@ int lcs_prim(famsa_ctx* ctx, int kind, int32_t* h_from, int32_t* h_to, double* h
         FB_CUDA(cudaMemcpyAsync(S.d_ids_a.p, S.h_quirky.data(), sizeof(uint32_t) * nq, cudaMemcpyHostToDevice, st));
         FB_TRY(lcs_rows(ctx, S.d_ids_a.as<uint32_t>(), S.h_quirky.data(), nq, nullptr, n, S.d_prim_side.p, 4, st));
     }
-    {   // (double) pow(i, 0.75), host libm, like Transform<double, indel075_div_lcs>'s table
-        std::vector<double> pw((size_t)2 * S.max_len + 2);
-        for (size_t v = 0; v < pw.size(); ++v) pw[v] = pow((double)v, 0.75);
-        FB_TRY(S.d_pow075_f64.reserve(sizeof(double) * pw.size()));
-        FB_CUDA(cudaMemcpyAsync(S.d_pow075_f64.p, pw.data(), sizeof(double) * pw.size(), cudaMemcpyHostToDevice, st));
-        FB_CUDA(cudaStreamSynchronize(st));
-    }
+    FB_TRY(lcs_pow075_f64(ctx, st));
     if (S.h_quirky.empty() && n >= 2 && !getenv("FAMSA_PRIM_SEQUENTIAL")) {
         const int rc = prim_boruvka(ctx, kind, eb, h_from, h_to, h_dist, h_order);
         if (rc != FAMSA_E_NOMEM) return rc;                         // no room for the float64 triangle: sequential loop

@@ -11,6 +11,7 @@
 //   CProfile::Align(p1, p2, ...)             src/core/profile.cpp:244                famsa_b200::AlignBatch(...)
 //   MSTPrim<>::run_view's vertex loop        src/tree/MSTPrim.cpp:280-549            CLCSBP::PrimEdges(...)
 //   CProfile(p1, p2) merge ctor, tables kept  profile.cpp:69-75, 784-1002            famsa_b200::ResidentProfiles
+//   DistanceCalculator<distance>::run        src/tree/DistanceCalculator.cpp:10-122   famsa_b200::ExportDistances(...)
 //     on the device between tree levels
 // Errors: the reference throws std::runtime_error and catches it in main() (src/famsa.cpp:160-165);
 // every non-zero C-ABI status is rethrown here the same way.  There is no CPU fallback.
@@ -19,6 +20,7 @@
 #include <cmath>
 #include <cstdint>
 #include <limits>
+#include <ostream>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -288,6 +290,28 @@ inline std::vector<std::pair<int, int>> UPGMATree(Context& ctx, Distance measure
     std::vector<std::pair<int, int>> out;
     for (uint32_t k = 0; k + 1 < n; ++k) out.emplace_back(t[2 * k], t[2 * k + 1]);
     return out;
+}
+
+// DistanceCalculator<distance>::run (DistanceCalculator.cpp:10-122) on the device: the -dist_export CSV of the set of
+// the last famsa_lcs_upload (input order) into `os`, byte for byte.  ids: CSequence::id without the leading '>'.
+// Returns the bytes written; a failing stream stops the export and throws.
+inline uint64_t ExportDistances(Context& ctx, const std::vector<std::string>& ids, Distance measure, bool square_matrix,
+                                std::ostream& os, uint64_t chunk_bytes = 0)
+{
+    std::string blob;
+    std::vector<uint64_t> offsets{0};
+    for (const std::string& id : ids) { blob += id; offsets.push_back(blob.size()); }
+    const bool pid = measure == Distance::pairwise_identity;
+    const int kind = measure == Distance::indel_div_lcs ? 1 : 0;
+    auto sink = [](void* user, const char* bytes, uint64_t n) -> int {
+        std::ostream& o = *static_cast<std::ostream*>(user);
+        o.write(bytes, (std::streamsize)n);
+        return o.good() ? 0 : 1;
+    };
+    uint64_t written = 0;
+    check(famsa_dist_export(ctx.get(), kind, square_matrix ? 1 : 0, pid ? 1 : 0, blob.data(), offsets.data(), chunk_bytes,
+                            sink, &os, &written));
+    return written;
 }
 
 // Level-synchronous order of the guide tree's merges (replaces CProfileQueue's one-at-a-time hand-out,

@@ -35,7 +35,8 @@ enum {
     FAMSA_E_NO_DEVICE = 2, /* no usable CUDA device (there is no CPU fallback) */
     FAMSA_E_CUDA = 3,      /* CUDA runtime / kernel failure */
     FAMSA_E_STATE = 4,     /* call order violated (e.g. LCS before upload) */
-    FAMSA_E_NOMEM = 5
+    FAMSA_E_NOMEM = 5,
+    FAMSA_E_SINK = 6       /* a caller's write callback refused bytes (famsa_dist_export) */
 };
 
 typedef struct famsa_ctx famsa_ctx;
@@ -182,6 +183,29 @@ int famsa_lcs_upgma(famsa_ctx* ctx, int distance_kind, int modified, int32_t* tr
  * writes it for rows 0..n_seqs) -- e.g. the triangle a multi-GPU run has just all-gathered. */
 int famsa_lcs_upgma_from_triangle(famsa_ctx* ctx, int distance_kind, int modified, const void* d_triangle, int elem_bytes,
                                   int32_t* tree);
+
+/* The distance-matrix export (-dist_export [-square_matrix] [-pid]): DistanceCalculator<distance>::run
+ * (src/tree/DistanceCalculator.cpp:10-122) with its text formatting, num2str / NumericConversions::Double2PChar
+ * (src/utils/conversion.h:52-119), on the device.  Works on the set of the last famsa_lcs_upload, in the caller's
+ * order (the reference exports in input order: no sorting, no duplicate removal, msa.cpp:518-526); after
+ * famsa_lcs_upload_sorted, or without a set, it returns FAMSA_E_STATE.
+ *   cell (r, c) = Transform(LCS with sequence r as the row (seq0), len_r, len_c) as float: pid != 0 gives
+ *   Transform<float, pairwise_identity> (distance_kind is then ignored), else Transform<double, distance_kind> rounded
+ *   to float (0 indel075_div_lcs, 1 indel_div_lcs).  square == 0: row r holds columns 0..r-1; square != 0: a header line
+ *   (',' + each id) and all n columns per row, the diagonal included (computed, and not symmetric in the dropped-carry
+ *   corner of lcsbp_classic.h:55-56).  Row text: id, ',', every value followed by ',', the last byte replaced by '\n'.
+ * ids: the FASTA headers without '>', id i = ids[id_offsets[i] .. id_offsets[i+1]) (n+1 offsets), written verbatim.
+ * The text is handed to `write` in order (header first), in chunks of whole rows of about chunk_bytes (0 = 32 MiB; a
+ * chunk grows to the widest row): the device formats and copies chunk k+1 while `write` consumes chunk k from a pinned
+ * buffer that stays valid until `write` returns.  `write` returns 0 to accept; anything else stops the call with
+ * FAMSA_E_SINK, no further writes, and a message naming the byte offset; the context stays usable.  `write` must not
+ * call into the same context.  *bytes_written (may be NULL) = bytes accepted.  The LCS triangle stays resident in HBM
+ * for the call; if it and the chunk buffers do not fit, FAMSA_E_NOMEM.  famsa_lcs_last_timing: total = all kernels of
+ * the call, main = the LCS tile kernels, n_pairs = cells exported. */
+typedef int (*famsa_write_fn)(void* user, const char* bytes, uint64_t n);        /* 0 = accepted */
+int famsa_dist_export(famsa_ctx* ctx, int distance_kind, int square, int pid,
+                      const char* ids, const uint64_t* id_offsets /* n+1 */, uint64_t chunk_bytes /* 0 = default */,
+                      famsa_write_fn write, void* user, uint64_t* bytes_written);
 
 /* Host-side Transform<T, Distance> (AbstractTreeGenerator.hpp:28-82), provided so bindings that
  * are not C++ get bit-identical distances.  kind: 0 indel075_div_lcs, 1 indel_div_lcs,
