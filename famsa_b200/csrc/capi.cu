@@ -37,6 +37,84 @@ using fb::set_error;
         return FAMSA_E_INVALID;                    \
     }
 
+// ------------------------------------------------------------------ the frame of an entry point
+
+// Reads the call's timing once its stream is synchronised: total = ev[0]..ev[3], main = ev[1]..ev[2]
+static int finish_timing(famsa_ctx* ctx, fb::CallTiming* t)
+{
+    FB_CUDA(cudaEventSynchronize(ctx->ev[3]));
+    FB_CUDA(cudaEventElapsedTime(&t->total_ms, ctx->ev[0], ctx->ev[3]));
+    FB_CUDA(cudaEventElapsedTime(&t->main_ms, ctx->ev[1], ctx->ev[2]));
+    return FAMSA_OK;
+}
+
+// Every entry point that queues work on the context's scratch: the NULL context, the lock, the argument checks (`check`,
+// before anything is queued), the device, the stream (the caller's, or the context's for NULL), the scratch order, then
+// `run`.  On a caller's stream the call returns with its work queued and the scratch held until that work is done; on the
+// context's stream it synchronises and, given `t`, reads the call's timing.
+using Timing = fb::CallTiming famsa_ctx::*;
+
+template <class Check, class Run>
+static int entry(famsa_ctx* ctx, void* stream, Timing t, Check check, Run run)
+{
+    FB_CHECK_CTX(ctx);
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    FB_TRY(check());
+    FB_CUDA(cudaSetDevice(ctx->device));
+    const cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+    FB_TRY(fb::scratch_acquire(ctx, st));
+    FB_TRY(run(st));
+    if (stream) return fb::scratch_release(ctx, st, false);
+    FB_CUDA(cudaStreamSynchronize(st));
+    fb::scratch_release(ctx, st, true);
+    return t ? finish_timing(ctx, &(ctx->*t)) : FAMSA_OK;
+}
+
+// An LCS call's events: ev[0] and ev[3] around all it queues; lcs_triangle and lcs_rows mark their tile kernels in ev[1]
+// and ev[2], and a call without any gets an empty span.
+template <class Run>
+static int lcs_timed(famsa_ctx* ctx, cudaStream_t st, Run run)
+{
+    ctx->lcs.tiles_marked = false;
+    FB_CUDA(cudaEventRecord(ctx->ev[0], st));
+    FB_TRY(run());
+    if (!ctx->lcs.tiles_marked) { FB_CUDA(cudaEventRecord(ctx->ev[1], st)); FB_CUDA(cudaEventRecord(ctx->ev[2], st)); }
+    FB_CUDA(cudaEventRecord(ctx->ev[3], st));
+    return FAMSA_OK;
+}
+
+static int check_set(const famsa_ctx* ctx, uint32_t min_n)
+{
+    if (ctx->lcs.n >= min_n) return FAMSA_OK;
+    set_error(ctx->lcs.n ? "the call needs at least " + std::to_string(min_n) + " uploaded sequences"
+                         : std::string("famsa_lcs_upload has not been called"));
+    return FAMSA_E_STATE;
+}
+
+// elem_bytes is 2 or 4 and at least `need` (LcsState::elem_bytes() for the LCS the library computes)
+static int check_elem(int elem_bytes, int need)
+{
+    if (elem_bytes != 2 && elem_bytes != 4) { set_error("elem_bytes must be 2 or 4"); return FAMSA_E_INVALID; }
+    if (elem_bytes < need) { set_error("elem_bytes == 2 needs every sequence shorter than 65536"); return FAMSA_E_INVALID; }
+    return FAMSA_OK;
+}
+
+static int check_rows(const famsa_ctx* ctx, uint32_t row_begin, uint32_t row_end)
+{
+    if (row_begin <= row_end && row_end <= ctx->lcs.n) return FAMSA_OK;
+    set_error("row range out of bounds");
+    return FAMSA_E_INVALID;
+}
+
+static int check_ids(const famsa_ctx* ctx, const uint32_t* ids, uint32_t count, const char* what)
+{
+    for (uint32_t k = 0; k < count; ++k)
+        if (ids[k] >= ctx->lcs.n) { set_error(std::string(what) + " id out of range"); return FAMSA_E_INVALID; }
+    return FAMSA_OK;
+}
+
+static uint64_t tri(uint64_t r) { return r ? r * (r - 1) / 2 : 0; }
+
 extern "C" {
 
 int famsa_abi_version(void) { return FAMSA_B200_ABI_VERSION; }
@@ -76,6 +154,9 @@ int famsa_create(int device, famsa_ctx** out_ctx)
         for (auto& e : ctx->ev_copy) FB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
         for (auto& e : ctx->ev_join) FB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
         for (auto& a : ctx->aux_stream) FB_CUDA(cudaStreamCreateWithFlags(&a, cudaStreamNonBlocking));
+        FB_CUDA(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
+        for (auto& e : ctx->ev_block) FB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        for (auto& e : ctx->ev_host) FB_CUDA(cudaEventCreate(&e));
         // per-call scratch and resident profiles are stream-ordered allocations: the pool keeps what it has
         cudaMemPool_t pool;
         FB_CUDA(cudaDeviceGetDefaultMemPool(&pool, device));
@@ -93,19 +174,9 @@ void famsa_destroy(famsa_ctx* ctx)
     if (!ctx) return;
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
-    fb::LcsState& S = ctx->lcs;
-    for (fb::DevBuf* b : {&S.d_perm, &S.d_invperm, &S.d_len_sorted, &S.d_code_off, &S.d_codes, &S.d_blob,
-                          &S.d_group_blob, &S.d_raw_codes, &S.d_raw_off, &S.d_raw_len, &S.d_flags, &S.d_pow075, &S.d_assign_lcs, &S.d_pow075_f64, &S.d_prim_tri, &S.d_prim_side, &S.d_prim_state,
-                          &S.d_prim_out, &S.d_prim_sideidx, &S.d_prim_cand, &S.d_prim_dtri, &S.d_prim_comp, &S.d_prim_best, &S.d_prim_part,
-                          &S.d_assign, &S.d_mind, &S.d_tiles,
-                          &S.d_res, &S.d_refpos, &S.d_ids_a, &S.d_ids_b, &S.d_out_stage, &S.d_masks64, &S.d_x64})
-        b->release();
     fb::dist_export_release(ctx);
     fb::prof_release_all(ctx);
-    fb::DpState& D = ctx->dp;
-    if (D.h_pinned) cudaFreeHost(D.h_pinned);
-    for (fb::DevBuf* b : {&D.d_dirs_out, &D.d_tables, &D.d_results, &D.d_path})
-        b->release();
+    if (ctx->dp.h_pinned) cudaFreeHost(ctx->dp.h_pinned);
     for (auto& ev : ctx->ev)
         if (ev) cudaEventDestroy(ev);
     for (auto& ev : ctx->ev_block)
@@ -124,7 +195,7 @@ void famsa_destroy(famsa_ctx* ctx)
         if (a) cudaStreamDestroy(a);
     if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
-    delete ctx;
+    delete ctx;                                                    // the device buffers free themselves
 }
 
 uint64_t famsa_kernel_launches(const famsa_ctx* ctx) { return ctx ? ctx->launches : 0; }
@@ -134,16 +205,15 @@ uint64_t famsa_kernel_launches(const famsa_ctx* ctx) { return ctx ? ctx->launche
 int famsa_lcs_upload(famsa_ctx* ctx, const int8_t* codes, const uint64_t* offsets, const uint32_t* lens,
                      uint32_t n_seqs)
 {
-    FB_CHECK_CTX(ctx);
-    if (n_seqs && (!codes || !offsets || !lens)) { set_error("NULL sequence arrays"); return FAMSA_E_INVALID; }
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    FB_CUDA(cudaSetDevice(ctx->device));
-    int rc = fb::scratch_acquire(ctx, ctx->stream);                 // earlier *_device calls may still read the old set
-    if (rc) return rc;
-    FB_CUDA(cudaStreamSynchronize(ctx->stream));
-    fb::scratch_release(ctx, ctx->stream, true);
-    ctx->lcs.h_order.clear();
-    return fb::lcs_upload(ctx, codes, offsets, lens, n_seqs);
+    return entry(ctx, nullptr, nullptr, [&]() -> int {
+        if (n_seqs && (!codes || !offsets || !lens)) { set_error("NULL sequence arrays"); return FAMSA_E_INVALID; }
+        return FAMSA_OK;
+    }, [&](cudaStream_t st) -> int {
+        FB_CUDA(cudaStreamSynchronize(st));                             // earlier *_device calls may still read the old set
+        fb::scratch_release(ctx, st, true);
+        ctx->lcs.h_order.clear();
+        return fb::lcs_upload(ctx, codes, offsets, lens, n_seqs);
+    });
 }
 
 int famsa_lcs_upload_sorted(famsa_ctx* ctx, const int8_t* codes, const uint64_t* offsets, const uint32_t* lens, uint32_t n_seqs)
@@ -182,112 +252,61 @@ uint64_t famsa_lcs_last_tiles(const famsa_ctx* ctx) { return ctx ? ctx->lcs.last
 
 uint32_t famsa_lcs_n_seqs(const famsa_ctx* ctx) { return ctx ? ctx->lcs.n : 0; }
 
-static int check_elem(const famsa_ctx* ctx, int elem_bytes)
-{
-    if (elem_bytes != 2 && elem_bytes != 4) { set_error("elem_bytes must be 2 or 4"); return FAMSA_E_INVALID; }
-    if (elem_bytes == 2 && ctx->lcs.max_len >= 65536) {
-        set_error("elem_bytes == 2 needs every sequence shorter than 65536");
-        return FAMSA_E_INVALID;
-    }
-    return FAMSA_OK;
-}
-
-static int finish_timing(famsa_ctx* ctx)
-{
-    float total = 0.f, main_ms = 0.f;
-    FB_CUDA(cudaEventSynchronize(ctx->ev[3]));
-    FB_CUDA(cudaEventElapsedTime(&total, ctx->ev[0], ctx->ev[3]));
-    FB_CUDA(cudaEventElapsedTime(&main_ms, ctx->ev[1], ctx->ev[2]));
-    ctx->lcs.last_total_ms = total;
-    ctx->lcs.last_main_ms = main_ms;
-    return FAMSA_OK;
-}
-
-static int triangle_locked(famsa_ctx* ctx, uint32_t row_begin, uint32_t row_end, void* d_out, int elem_bytes,
-                           void* stream)
-{
-    if (ctx->lcs.n == 0 && row_end > 0) { set_error("famsa_lcs_upload has not been called"); return FAMSA_E_STATE; }
-    if (row_begin > row_end || row_end > ctx->lcs.n) { set_error("row range out of bounds"); return FAMSA_E_INVALID; }
-    int rc = check_elem(ctx, elem_bytes);
-    if (rc) return rc;
-    if (!d_out && row_end > row_begin && row_end > 1) { set_error("d_out is NULL"); return FAMSA_E_INVALID; }
-    FB_CUDA(cudaSetDevice(ctx->device));
-    cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
-    if ((rc = fb::scratch_acquire(ctx, st))) return rc;
-    rc = fb::lcs_triangle(ctx, row_begin, row_end, d_out, elem_bytes, st);
-    if (rc) return rc;
-    if (!stream) { FB_CUDA(cudaStreamSynchronize(st)); fb::scratch_release(ctx, st, true); return finish_timing(ctx); }
-    return fb::scratch_release(ctx, st, false);
-}
-
 int famsa_lcs_triangle_device(famsa_ctx* ctx, uint32_t row_begin, uint32_t row_end, void* d_out, int elem_bytes,
                               void* stream)
 {
-    FB_CHECK_CTX(ctx);
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    return triangle_locked(ctx, row_begin, row_end, d_out, elem_bytes, stream);
+    return entry(ctx, stream, &famsa_ctx::lcs_timing, [&]() -> int {
+        FB_TRY(check_set(ctx, row_end > 0 ? 1 : 0));
+        FB_TRY(check_rows(ctx, row_begin, row_end));
+        FB_TRY(check_elem(elem_bytes, ctx->lcs.elem_bytes()));
+        if (!d_out && row_end > row_begin && row_end > 1) { set_error("d_out is NULL"); return FAMSA_E_INVALID; }
+        return FAMSA_OK;
+    }, [&](cudaStream_t st) -> int {
+        ctx->lcs.last_pairs = tri(row_end) - tri(row_begin);
+        return lcs_timed(ctx, st, [&] { return fb::lcs_triangle(ctx, row_begin, row_end, d_out, elem_bytes, st); });
+    });
 }
 
 int famsa_lcs_triangle(famsa_ctx* ctx, uint32_t row_begin, uint32_t row_end, void* out, int elem_bytes)
 {
-    FB_CHECK_CTX(ctx);
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    if (row_begin > row_end || row_end > ctx->lcs.n) { set_error("row range out of bounds"); return FAMSA_E_INVALID; }
-    if (elem_bytes != 2 && elem_bytes != 4) { set_error("elem_bytes must be 2 or 4"); return FAMSA_E_INVALID; }
-    auto tri = [](uint64_t r) { return r ? r * (r - 1) / 2 : 0; };
     const uint64_t pairs = tri(row_end) - tri(row_begin);
-    if (pairs && !out) { set_error("out is NULL"); return FAMSA_E_INVALID; }
-    FB_CUDA(cudaSetDevice(ctx->device));
-    int rc = ctx->lcs.d_out_stage.reserve(std::max<uint64_t>(pairs, 1) * elem_bytes);
-    if (rc) return rc;
-    char* d_out = static_cast<char*>(ctx->lcs.d_out_stage.p);
-
-    // Row blocks with equal numbers of pairs: all kernels are queued first, then every block is copied back as
-    // soon as its event fires, so the D2H of block k overlaps the kernels of blocks k+1...
-    constexpr int kBlocks = 8;
-    // (worth it only when the copy is long compared with the tail of a kernel: hundreds of millions of pairs)
-    unsigned long long block_min = 400000000ull;
-    if (const char* e = getenv("FAMSA_LCS_BLOCK_MIN_PAIRS")) block_min = strtoull(e, nullptr, 10);   // test knob
-    const int n_blocks = (ctx->lcs.identity_perm && pairs > block_min) ? kBlocks : 1;
-    uint32_t bounds[kBlocks + 1];
-    bounds[0] = row_begin;
-    for (int b = 1; b < n_blocks; ++b) {
-        const double target = (double)tri(row_begin) + (double)pairs * b / n_blocks;
-        uint32_t r = (uint32_t)((1.0 + std::sqrt(1.0 + 8.0 * target)) / 2.0);
-        r = (r + 16) / 32 * 32;                                        // on a mask-group boundary: no group is computed twice
-        bounds[b] = std::min(std::max(r, bounds[b - 1]), row_end);
-    }
-    bounds[n_blocks] = row_end;
-    if (!ctx->copy_stream) {
-        FB_CUDA(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
-        for (auto& e : ctx->ev_block) FB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        for (auto& e : ctx->ev_host) FB_CUDA(cudaEventCreate(&e));
-    }
-    if (ctx->lcs.n == 0 && row_end > 0) { set_error("famsa_lcs_upload has not been called"); return FAMSA_E_STATE; }
-    rc = check_elem(ctx, elem_bytes);
-    if (rc) return rc;
-    if ((rc = fb::scratch_acquire(ctx, ctx->stream))) return rc;
-    FB_CUDA(cudaEventRecord(ctx->ev_host[0], ctx->stream));
-    float main_ms = 0.f;
-    rc = fb::lcs_triangle(ctx, row_begin, row_end, d_out, elem_bytes, ctx->stream, bounds, n_blocks, ctx->ev_block, true, true);
-    if (rc) return rc;
-    if (!ctx->lcs.identity_perm && n_blocks == 1) FB_CUDA(cudaEventRecord(ctx->ev_block[0], ctx->stream));
-    FB_CUDA(cudaEventRecord(ctx->ev_host[1], ctx->stream));
-    for (int b = 0; b < n_blocks; ++b) {
-        const uint64_t off = (tri(bounds[b]) - tri(row_begin)) * elem_bytes;
-        const uint64_t bytes = (tri(bounds[b + 1]) - tri(bounds[b])) * elem_bytes;
-        if (!bytes) continue;
-        FB_CUDA(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_block[b], 0));
-        FB_CUDA(cudaMemcpyAsync(static_cast<char*>(out) + off, d_out + off, bytes, cudaMemcpyDeviceToHost, ctx->copy_stream));
-    }
-    FB_CUDA(cudaStreamSynchronize(ctx->stream));
-    FB_CUDA(cudaStreamSynchronize(ctx->copy_stream));
-    fb::scratch_release(ctx, ctx->stream, true);
-    FB_CUDA(cudaEventElapsedTime(&main_ms, ctx->ev_host[0], ctx->ev_host[1]));
-    ctx->lcs.last_total_ms = main_ms;
-    ctx->lcs.last_main_ms = main_ms;
-    ctx->lcs.last_pairs = pairs;
-    return FAMSA_OK;
+    return entry(ctx, nullptr, nullptr, [&]() -> int {
+        FB_TRY(check_rows(ctx, row_begin, row_end));
+        FB_TRY(check_elem(elem_bytes, ctx->lcs.elem_bytes()));
+        if (pairs && !out) { set_error("out is NULL"); return FAMSA_E_INVALID; }
+        return FAMSA_OK;
+    }, [&](cudaStream_t st) -> int {
+        fb::LcsState& S = ctx->lcs;
+        FB_TRY(S.d_out_stage.reserve(std::max<uint64_t>(pairs, 1) * elem_bytes));
+        char* d_out = static_cast<char*>(S.d_out_stage.p);
+        // Row blocks with equal numbers of pairs: all kernels are queued first, then every block is copied back as
+        // soon as its event fires, so the D2H of block k overlaps the kernels of blocks k+1...
+        constexpr int kBlocks = 8;
+        // (worth it only when the copy is long compared with the tail of a kernel: hundreds of millions of pairs)
+        unsigned long long block_min = 400000000ull;
+        if (const char* e = getenv("FAMSA_LCS_BLOCK_MIN_PAIRS")) block_min = strtoull(e, nullptr, 10);   // test knob
+        const int n_blocks = (S.identity_perm && pairs > block_min) ? kBlocks : 1;
+        uint32_t bounds[kBlocks + 1];
+        fb::lcs_row_pieces(row_begin, row_end, n_blocks, nullptr, bounds);
+        FB_CUDA(cudaEventRecord(ctx->ev_host[0], st));
+        FB_TRY(fb::lcs_triangle(ctx, row_begin, row_end, d_out, elem_bytes, st, bounds, n_blocks, ctx->ev_block, true, true));
+        if (!S.identity_perm && n_blocks == 1) FB_CUDA(cudaEventRecord(ctx->ev_block[0], st));
+        FB_CUDA(cudaEventRecord(ctx->ev_host[1], st));
+        for (int b = 0; b < n_blocks; ++b) {
+            const uint64_t off = (tri(bounds[b]) - tri(row_begin)) * elem_bytes;
+            const uint64_t bytes = (tri(bounds[b + 1]) - tri(bounds[b])) * elem_bytes;
+            if (!bytes) continue;
+            FB_CUDA(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_block[b], 0));
+            FB_CUDA(cudaMemcpyAsync(static_cast<char*>(out) + off, d_out + off, bytes, cudaMemcpyDeviceToHost, ctx->copy_stream));
+        }
+        FB_CUDA(cudaStreamSynchronize(st));
+        FB_CUDA(cudaStreamSynchronize(ctx->copy_stream));
+        // its own timing: the kernels of all blocks, their copies overlapped
+        FB_CUDA(cudaEventElapsedTime(&ctx->lcs_timing.main_ms, ctx->ev_host[0], ctx->ev_host[1]));
+        ctx->lcs_timing.total_ms = ctx->lcs_timing.main_ms;
+        S.last_pairs = pairs;
+        return FAMSA_OK;
+    });
 }
 
 // ------------------------------------------------------------------ multi-GPU exchange over peer memory
@@ -348,46 +367,31 @@ int famsa_ipc_close(famsa_ctx* ctx, void* d_ptr)
 int famsa_lcs_triangle_exchange(famsa_ctx* ctx, uint32_t row_begin, uint32_t row_end, void* d_full, void* const* d_peer_full,
                                 uint32_t n_peers, int elem_bytes, uint32_t n_pieces, void* stream)
 {
-    FB_CHECK_CTX(ctx);
-    std::lock_guard<std::mutex> lk(ctx->mu);
     constexpr uint32_t kPieces = sizeof(ctx->ev_block) / sizeof(ctx->ev_block[0]);
-    if (ctx->lcs.n == 0) { set_error("famsa_lcs_upload has not been called"); return FAMSA_E_STATE; }
-    if (row_begin > row_end || row_end > ctx->lcs.n) { set_error("row range out of bounds"); return FAMSA_E_INVALID; }
-    if (!d_full || (n_peers && !d_peer_full)) { set_error("NULL triangle buffer"); return FAMSA_E_INVALID; }
-    for (uint32_t k = 0; k < n_peers; ++k)
-        if (!d_peer_full[k]) { set_error("NULL peer buffer"); return FAMSA_E_INVALID; }
-    int rc = check_elem(ctx, elem_bytes);
-    if (rc) return rc;
-    FB_CUDA(cudaSetDevice(ctx->device));
-    cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
-    if (!ctx->copy_stream) {
-        FB_CUDA(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
-        for (auto& e : ctx->ev_block) FB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        for (auto& e : ctx->ev_host) FB_CUDA(cudaEventCreate(&e));
-    }
-    auto tri = [](uint64_t r) { return r ? r * (r - 1) / 2 : 0; };
-    // Pieces (a non-identity order cannot be cut by rows: one piece).  The copy of the LAST piece is the only exposed part of
-    // the exchange, so the pieces shrink towards the end: 14 % of the pairs each at first, 8 % at last.
-    const uint32_t np = ctx->lcs.identity_perm ? std::min(std::max(n_pieces, 1u), kPieces) : 1u;
-    uint32_t bounds[kPieces + 1];
-    bounds[0] = row_begin;
-    const uint64_t pairs = tri(row_end) - tri(row_begin);
-    static const double kCut8[9] = {0.0, 0.14, 0.28, 0.42, 0.56, 0.70, 0.82, 0.92, 1.0};
-    for (uint32_t b = 1; b < np; ++b) {
-        const double frac = np == 8 ? kCut8[b] : (double)b / np;
-        const double target = (double)tri(row_begin) + (double)pairs * frac;
-        uint32_t r = (uint32_t)((1.0 + std::sqrt(1.0 + 8.0 * target)) / 2.0);
-        r = (r + 16) / 32 * 32;                                        // on a mask-group boundary: no group is computed twice
-        bounds[b] = std::min(std::max(r, bounds[b - 1]), row_end);
-    }
-    bounds[np] = row_end;
-    if ((rc = fb::scratch_acquire(ctx, st))) return rc;
-    char* own = static_cast<char*>(d_full) + tri(row_begin) * elem_bytes;    // lcs_triangle indexes from its first row
-    rc = fb::lcs_triangle(ctx, row_begin, row_end, own, elem_bytes, st, bounds, (int)np, ctx->ev_block, true, true);
-    if (rc) return rc;
-    // every finished piece goes to the same place of every peer's triangle while the next pieces are being computed: copy
-    // engines over NVLink, no SM and no collective kernel involved
-    if (n_peers) {
+    return entry(ctx, stream, &famsa_ctx::lcs_timing, [&]() -> int {
+        FB_TRY(check_set(ctx, 1));
+        FB_TRY(check_rows(ctx, row_begin, row_end));
+        if (!d_full || (n_peers && !d_peer_full)) { set_error("NULL triangle buffer"); return FAMSA_E_INVALID; }
+        for (uint32_t k = 0; k < n_peers; ++k)
+            if (!d_peer_full[k]) { set_error("NULL peer buffer"); return FAMSA_E_INVALID; }
+        return check_elem(elem_bytes, ctx->lcs.elem_bytes());
+    }, [&](cudaStream_t st) -> int {
+        // Pieces (a non-identity order cannot be cut by rows: one piece).  The copy of the LAST piece is the only exposed part
+        // of the exchange, so the pieces shrink towards the end: 14 % of the pairs each at first, 8 % at last.
+        const uint32_t np = ctx->lcs.identity_perm ? std::min(std::max(n_pieces, 1u), kPieces) : 1u;
+        static const double kCut8[9] = {0.0, 0.14, 0.28, 0.42, 0.56, 0.70, 0.82, 0.92, 1.0};
+        double frac[kPieces + 1];
+        for (uint32_t b = 0; b <= np; ++b) frac[b] = np == 8 ? kCut8[b] : (double)b / np;
+        uint32_t bounds[kPieces + 1];
+        fb::lcs_row_pieces(row_begin, row_end, (int)np, frac, bounds);
+        ctx->lcs.last_pairs = tri(row_end) - tri(row_begin);
+        char* own = static_cast<char*>(d_full) + tri(row_begin) * elem_bytes;    // lcs_triangle indexes from its first row
+        FB_TRY(lcs_timed(ctx, st, [&] {
+            return fb::lcs_triangle(ctx, row_begin, row_end, own, elem_bytes, st, bounds, (int)np, ctx->ev_block, true, true);
+        }));
+        // every finished piece goes to the same place of every peer's triangle while the next pieces are being computed:
+        // copy engines over NVLink, no SM and no collective kernel involved
+        if (!n_peers) return FAMSA_OK;
         constexpr int kLanes = 1 + sizeof(ctx->peer_stream) / sizeof(ctx->peer_stream[0]);
         cudaStream_t lanes[kLanes];
         lanes[0] = ctx->copy_stream;
@@ -408,180 +412,141 @@ int famsa_lcs_triangle_exchange(famsa_ctx* ctx, uint32_t row_begin, uint32_t row
             FB_CUDA(cudaEventRecord(ctx->ev_copy[a], lanes[a]));
             FB_CUDA(cudaStreamWaitEvent(st, ctx->ev_copy[a], 0));
         }
-    }
-    if (!stream) { FB_CUDA(cudaStreamSynchronize(st)); fb::scratch_release(ctx, st, true); return finish_timing(ctx); }
-    return fb::scratch_release(ctx, st, false);
-}
-
-static int rows_common(famsa_ctx* ctx, const uint32_t* d_ref_ids, const uint32_t* h_ref_ids, uint32_t n_ref,
-                       const uint32_t* d_col_ids, uint32_t n_col, void* d_out, int elem_bytes, void* stream)
-{
-    cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
-    for (uint32_t r = 0; r < n_ref; ++r)
-        if (h_ref_ids[r] >= ctx->lcs.n) { set_error("ref id out of range"); return FAMSA_E_INVALID; }
-    int rc = fb::scratch_acquire(ctx, st);
-    if (rc) return rc;
-    rc = fb::lcs_rows(ctx, d_ref_ids, h_ref_ids, n_ref, d_col_ids, n_col, d_out, elem_bytes, st);
-    if (rc) return rc;
-    if (!stream) { FB_CUDA(cudaStreamSynchronize(st)); fb::scratch_release(ctx, st, true); return finish_timing(ctx); }
-    return fb::scratch_release(ctx, st, false);
+        return FAMSA_OK;
+    });
 }
 
 int famsa_lcs_rows_device(famsa_ctx* ctx, const uint32_t* d_ref_ids, uint32_t n_ref, const uint32_t* d_col_ids,
                           uint32_t n_col, void* d_out, int elem_bytes, void* stream)
 {
-    FB_CHECK_CTX(ctx);
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    if (ctx->lcs.n == 0) { set_error("famsa_lcs_upload has not been called"); return FAMSA_E_STATE; }
-    int rc = check_elem(ctx, elem_bytes);
-    if (rc) return rc;
-    if (!d_col_ids && n_col > ctx->lcs.n) { set_error("n_col exceeds the number of sequences"); return FAMSA_E_INVALID; }
-    if (n_ref && !d_ref_ids) { set_error("d_ref_ids is NULL"); return FAMSA_E_INVALID; }
-    FB_CUDA(cudaSetDevice(ctx->device));
     std::vector<uint32_t> h_ref(n_ref);
-    if (n_ref) {      // ordered on the caller's stream (a blocking copy on the legacy stream would not be)
-        cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
-        FB_CUDA(cudaMemcpyAsync(h_ref.data(), d_ref_ids, sizeof(uint32_t) * n_ref, cudaMemcpyDeviceToHost, st));
-        FB_CUDA(cudaStreamSynchronize(st));
-    }
-    return rows_common(ctx, d_ref_ids, h_ref.data(), n_ref, d_col_ids, n_col, d_out, elem_bytes, stream);
+    return entry(ctx, stream, &famsa_ctx::lcs_timing, [&]() -> int {
+        FB_TRY(check_set(ctx, 1));
+        FB_TRY(check_elem(elem_bytes, ctx->lcs.elem_bytes()));
+        if (!d_col_ids && n_col > ctx->lcs.n) { set_error("n_col exceeds the number of sequences"); return FAMSA_E_INVALID; }
+        if (n_ref && !d_ref_ids) { set_error("d_ref_ids is NULL"); return FAMSA_E_INVALID; }
+        if (n_ref) {      // ordered on the caller's stream (a blocking copy on the legacy stream would not be)
+            FB_CUDA(cudaSetDevice(ctx->device));
+            cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+            FB_CUDA(cudaMemcpyAsync(h_ref.data(), d_ref_ids, sizeof(uint32_t) * n_ref, cudaMemcpyDeviceToHost, st));
+            FB_CUDA(cudaStreamSynchronize(st));
+        }
+        return check_ids(ctx, h_ref.data(), n_ref, "ref");
+    }, [&](cudaStream_t st) -> int {
+        ctx->lcs.last_pairs = (uint64_t)n_ref * n_col;
+        return lcs_timed(ctx, st, [&] { return fb::lcs_rows(ctx, h_ref.data(), n_ref, d_col_ids, n_col, d_out, elem_bytes, st); });
+    });
 }
 
 int famsa_lcs_rows(famsa_ctx* ctx, const uint32_t* ref_ids, uint32_t n_ref, const uint32_t* col_ids, uint32_t n_col,
                    void* out, int elem_bytes)
 {
-    FB_CHECK_CTX(ctx);
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    if (ctx->lcs.n == 0) { set_error("famsa_lcs_upload has not been called"); return FAMSA_E_STATE; }
-    int rc = check_elem(ctx, elem_bytes);
-    if (rc) return rc;
-    if (!col_ids && n_col > ctx->lcs.n) { set_error("n_col exceeds the number of sequences"); return FAMSA_E_INVALID; }
-    if ((n_ref && !ref_ids) || (n_ref && n_col && !out)) { set_error("NULL argument"); return FAMSA_E_INVALID; }
-    if (col_ids)
-        for (uint32_t k = 0; k < n_col; ++k)
-            if (col_ids[k] >= ctx->lcs.n) { set_error("col id out of range"); return FAMSA_E_INVALID; }
-    FB_CUDA(cudaSetDevice(ctx->device));
-    fb::LcsState& S = ctx->lcs;
-    const uint64_t cells = (uint64_t)n_ref * n_col;
-    rc = S.d_out_stage.reserve(std::max<uint64_t>(cells, 1) * elem_bytes);
-    if (rc) return rc;
-    rc = S.d_ids_a.reserve(sizeof(uint32_t) * std::max(1u, n_ref));
-    if (rc) return rc;
-    const uint32_t* d_cols = nullptr;
-    if (col_ids) {
-        rc = S.d_ids_b.reserve(sizeof(uint32_t) * std::max(1u, n_col));
-        if (rc) return rc;
-        FB_CUDA(cudaMemcpyAsync(S.d_ids_b.p, col_ids, sizeof(uint32_t) * n_col, cudaMemcpyHostToDevice, ctx->stream));
-        d_cols = S.d_ids_b.as<uint32_t>();
-    }
-    if (n_ref)
-        FB_CUDA(cudaMemcpyAsync(S.d_ids_a.p, ref_ids, sizeof(uint32_t) * n_ref, cudaMemcpyHostToDevice, ctx->stream));
-    rc = rows_common(ctx, S.d_ids_a.as<uint32_t>(), ref_ids, n_ref, d_cols, n_col, S.d_out_stage.p, elem_bytes, nullptr);
-    if (rc) return rc;
-    if (cells) FB_CUDA(cudaMemcpy(out, S.d_out_stage.p, cells * elem_bytes, cudaMemcpyDeviceToHost));
-    return FAMSA_OK;
+    return entry(ctx, nullptr, &famsa_ctx::lcs_timing, [&]() -> int {
+        FB_TRY(check_set(ctx, 1));
+        FB_TRY(check_elem(elem_bytes, ctx->lcs.elem_bytes()));
+        if (!col_ids && n_col > ctx->lcs.n) { set_error("n_col exceeds the number of sequences"); return FAMSA_E_INVALID; }
+        if ((n_ref && !ref_ids) || (n_ref && n_col && !out)) { set_error("NULL argument"); return FAMSA_E_INVALID; }
+        if (col_ids) FB_TRY(check_ids(ctx, col_ids, n_col, "col"));
+        return check_ids(ctx, ref_ids, n_ref, "ref");
+    }, [&](cudaStream_t st) -> int {
+        fb::LcsState& S = ctx->lcs;
+        const uint64_t cells = (uint64_t)n_ref * n_col;
+        FB_TRY(S.d_out_stage.reserve(std::max<uint64_t>(cells, 1) * elem_bytes));
+        const uint32_t* d_cols = nullptr;
+        if (col_ids) {
+            FB_TRY(S.d_ids_b.reserve(sizeof(uint32_t) * std::max(1u, n_col)));
+            FB_CUDA(cudaMemcpyAsync(S.d_ids_b.p, col_ids, sizeof(uint32_t) * n_col, cudaMemcpyHostToDevice, st));
+            d_cols = S.d_ids_b.as<uint32_t>();
+        }
+        S.last_pairs = cells;
+        FB_TRY(lcs_timed(ctx, st, [&] { return fb::lcs_rows(ctx, ref_ids, n_ref, d_cols, n_col, S.d_out_stage.p, elem_bytes, st); }));
+        if (cells) FB_CUDA(cudaMemcpyAsync(out, S.d_out_stage.p, cells * elem_bytes, cudaMemcpyDeviceToHost, st));
+        return FAMSA_OK;
+    });
 }
 
 int famsa_lcs_prim(famsa_ctx* ctx, int distance_kind, int32_t* edge_from, int32_t* edge_to, double* edge_dist,
                    int32_t* prim_order)
 {
-    FB_CHECK_CTX(ctx);
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    if (ctx->lcs.n == 0) { set_error("famsa_lcs_upload has not been called"); return FAMSA_E_STATE; }
-    if (!prim_order || (ctx->lcs.n > 1 && (!edge_from || !edge_to || !edge_dist))) { set_error("NULL argument"); return FAMSA_E_INVALID; }
-    if (distance_kind != 0 && distance_kind != 1) { set_error("MSTPrim is instantiated for distance_kind 0 and 1 only"); return FAMSA_E_INVALID; }
-    FB_CUDA(cudaSetDevice(ctx->device));
-    int rc = fb::scratch_acquire(ctx, ctx->stream);
-    if (rc) return rc;
-    rc = fb::lcs_prim(ctx, distance_kind, edge_from, edge_to, edge_dist, prim_order);
-    if (rc) return rc;
-    FB_CUDA(cudaStreamSynchronize(ctx->stream));
-    fb::scratch_release(ctx, ctx->stream, true);
-    return finish_timing(ctx);
+    std::vector<fb::MstEdge> tree;
+    const int rc = entry(ctx, nullptr, &famsa_ctx::lcs_timing, [&]() -> int {
+        FB_TRY(check_set(ctx, 1));
+        if (!prim_order || (ctx->lcs.n > 1 && (!edge_from || !edge_to || !edge_dist))) { set_error("NULL argument"); return FAMSA_E_INVALID; }
+        if (distance_kind != 0 && distance_kind != 1) { set_error("MSTPrim is instantiated for distance_kind 0 and 1 only"); return FAMSA_E_INVALID; }
+        return FAMSA_OK;
+    }, [&](cudaStream_t st) -> int {
+        ctx->lcs.last_pairs = tri(ctx->lcs.n);
+        return lcs_timed(ctx, st, [&] { return fb::lcs_prim(ctx, distance_kind, edge_from, edge_to, edge_dist, prim_order, tree); });
+    });
+    if (rc || tree.empty()) return rc;
+    return fb::prim_replay(tree, edge_from, edge_to, edge_dist, prim_order);     // host only: outside the call's timing
 }
 
 int famsa_lcs_assign(famsa_ctx* ctx, const uint32_t* seed_ids, uint32_t n_seeds, int distance_kind, uint32_t* assignments,
                      float* min_dist)
 {
-    FB_CHECK_CTX(ctx);
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    if (ctx->lcs.n == 0) { set_error("famsa_lcs_upload has not been called"); return FAMSA_E_STATE; }
-    if (!seed_ids || !n_seeds || !assignments || !min_dist) { set_error("NULL argument / no seeds"); return FAMSA_E_INVALID; }
-    if (distance_kind < 0 || distance_kind > 2) { set_error("distance_kind must be 0, 1 or 2"); return FAMSA_E_INVALID; }
-    for (uint32_t k = 0; k < n_seeds; ++k)
-        if (seed_ids[k] >= ctx->lcs.n) { set_error("seed id out of range"); return FAMSA_E_INVALID; }
-    FB_CUDA(cudaSetDevice(ctx->device));
-    int rc = fb::scratch_acquire(ctx, ctx->stream);
-    if (rc) return rc;
-    rc = fb::lcs_assign(ctx, seed_ids, n_seeds, distance_kind, assignments, min_dist);
-    if (rc) return rc;
-    FB_CUDA(cudaStreamSynchronize(ctx->stream));
-    fb::scratch_release(ctx, ctx->stream, true);
-    return finish_timing(ctx);
+    return entry(ctx, nullptr, &famsa_ctx::lcs_timing, [&]() -> int {
+        FB_TRY(check_set(ctx, 1));
+        if (!seed_ids || !n_seeds || !assignments || !min_dist) { set_error("NULL argument / no seeds"); return FAMSA_E_INVALID; }
+        if (distance_kind < 0 || distance_kind > 2) { set_error("distance_kind must be 0, 1 or 2"); return FAMSA_E_INVALID; }
+        return check_ids(ctx, seed_ids, n_seeds, "seed");
+    }, [&](cudaStream_t st) -> int {
+        ctx->lcs.last_pairs = (uint64_t)n_seeds * ctx->lcs.n;
+        return lcs_timed(ctx, st, [&] { return fb::lcs_assign(ctx, seed_ids, n_seeds, distance_kind, assignments, min_dist); });
+    });
 }
 
 int famsa_lcs_upgma(famsa_ctx* ctx, int distance_kind, int modified, int32_t* tree)
 {
-    FB_CHECK_CTX(ctx);
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    if (ctx->lcs.n < 2) { set_error("famsa_lcs_upgma needs at least two uploaded sequences"); return FAMSA_E_STATE; }
-    if (!tree) { set_error("NULL argument"); return FAMSA_E_INVALID; }
-    if (distance_kind < 0 || distance_kind > 2) { set_error("distance_kind must be 0, 1 or 2"); return FAMSA_E_INVALID; }
-    FB_CUDA(cudaSetDevice(ctx->device));
-    int rc = fb::scratch_acquire(ctx, ctx->stream);
-    if (rc) return rc;
-    rc = fb::lcs_upgma(ctx, distance_kind, modified, tree);
-    if (rc) return rc;
-    fb::scratch_release(ctx, ctx->stream, true);
-    return finish_timing(ctx);
+    return entry(ctx, nullptr, &famsa_ctx::lcs_timing, [&]() -> int {
+        FB_TRY(check_set(ctx, 2));
+        if (!tree) { set_error("NULL argument"); return FAMSA_E_INVALID; }
+        if (distance_kind < 0 || distance_kind > 2) { set_error("distance_kind must be 0, 1 or 2"); return FAMSA_E_INVALID; }
+        return FAMSA_OK;
+    }, [&](cudaStream_t st) -> int {
+        ctx->lcs.last_pairs = tri(ctx->lcs.n);
+        return lcs_timed(ctx, st, [&] { return fb::lcs_upgma(ctx, distance_kind, modified, tree); });
+    });
 }
 
 int famsa_lcs_upgma_from_triangle(famsa_ctx* ctx, int distance_kind, int modified, const void* d_triangle, int elem_bytes, int32_t* tree)
 {
-    FB_CHECK_CTX(ctx);
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    if (ctx->lcs.n < 2) { set_error("famsa_lcs_upgma needs at least two uploaded sequences"); return FAMSA_E_STATE; }
-    if (!tree || !d_triangle) { set_error("NULL argument"); return FAMSA_E_INVALID; }
-    if (distance_kind < 0 || distance_kind > 2) { set_error("distance_kind must be 0, 1 or 2"); return FAMSA_E_INVALID; }
-    if (elem_bytes != 2 && elem_bytes != 4) { set_error("elem_bytes must be 2 or 4"); return FAMSA_E_INVALID; }
-    FB_CUDA(cudaSetDevice(ctx->device));
-    int rc = fb::scratch_acquire(ctx, ctx->stream);
-    if (rc) return rc;
-    rc = fb::lcs_upgma(ctx, distance_kind, modified, tree, d_triangle, elem_bytes);
-    if (rc) return rc;
-    fb::scratch_release(ctx, ctx->stream, true);
-    return finish_timing(ctx);
+    return entry(ctx, nullptr, &famsa_ctx::lcs_timing, [&]() -> int {
+        FB_TRY(check_set(ctx, 2));
+        if (!tree || !d_triangle) { set_error("NULL argument"); return FAMSA_E_INVALID; }
+        if (distance_kind < 0 || distance_kind > 2) { set_error("distance_kind must be 0, 1 or 2"); return FAMSA_E_INVALID; }
+        return check_elem(elem_bytes, 2);                               // the caller's triangle: any width the caller chose
+    }, [&](cudaStream_t st) -> int {
+        ctx->lcs.last_pairs = 0;
+        return lcs_timed(ctx, st, [&] { return fb::lcs_upgma(ctx, distance_kind, modified, tree, d_triangle, elem_bytes); });
+    });
 }
 
 int famsa_lcs_assign_shard(famsa_ctx* ctx, const uint32_t* seed_ids, uint32_t n_seeds, int distance_kind, uint32_t shard,
                            uint32_t n_shards, int64_t* d_packed, void* stream)
 {
-    FB_CHECK_CTX(ctx);
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    if (ctx->lcs.n == 0) { set_error("famsa_lcs_upload has not been called"); return FAMSA_E_STATE; }
-    if (!seed_ids || !n_seeds || !d_packed) { set_error("NULL argument / no seeds"); return FAMSA_E_INVALID; }
-    if (distance_kind < 0 || distance_kind > 2) { set_error("distance_kind must be 0, 1 or 2"); return FAMSA_E_INVALID; }
-    if (!n_shards || shard >= n_shards) { set_error("shard out of range"); return FAMSA_E_INVALID; }
-    for (uint32_t k = 0; k < n_seeds; ++k)
-        if (seed_ids[k] >= ctx->lcs.n) { set_error("seed id out of range"); return FAMSA_E_INVALID; }
-    FB_CUDA(cudaSetDevice(ctx->device));
-    cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
-    int rc = fb::scratch_acquire(ctx, st);
-    if (rc) return rc;
-    rc = fb::lcs_assign_shard(ctx, seed_ids, n_seeds, distance_kind, shard, n_shards, reinterpret_cast<long long*>(d_packed), st);
-    if (rc) return rc;
-    if (!stream) { FB_CUDA(cudaStreamSynchronize(st)); fb::scratch_release(ctx, st, true); return finish_timing(ctx); }
-    // the seed ids were handed to an async copy from pageable memory: staged by the driver before the call returned
-    return fb::scratch_release(ctx, st, false);
+    // (the seed ids are handed to an async copy from pageable memory: staged by the driver before the call returns)
+    return entry(ctx, stream, &famsa_ctx::lcs_timing, [&]() -> int {
+        FB_TRY(check_set(ctx, 1));
+        if (!seed_ids || !n_seeds || !d_packed) { set_error("NULL argument / no seeds"); return FAMSA_E_INVALID; }
+        if (distance_kind < 0 || distance_kind > 2) { set_error("distance_kind must be 0, 1 or 2"); return FAMSA_E_INVALID; }
+        if (!n_shards || shard >= n_shards) { set_error("shard out of range"); return FAMSA_E_INVALID; }
+        return check_ids(ctx, seed_ids, n_seeds, "seed");
+    }, [&](cudaStream_t st) -> int {
+        return lcs_timed(ctx, st, [&] {
+            return fb::lcs_assign_shard(ctx, seed_ids, n_seeds, distance_kind, shard, n_shards, reinterpret_cast<long long*>(d_packed), st);
+        });
+    });
 }
 
+// Not through entry(): the export keeps its own timing and gives the scratch back even when it fails.
 int famsa_dist_export(famsa_ctx* ctx, int distance_kind, int square, int pid, const char* ids, const uint64_t* id_offsets,
                       uint64_t chunk_bytes, famsa_write_fn write, void* user, uint64_t* bytes_written)
 {
     FB_CHECK_CTX(ctx);
     std::lock_guard<std::mutex> lk(ctx->mu);
     if (bytes_written) *bytes_written = 0;
-    if (ctx->lcs.n == 0) { set_error("famsa_dist_export: famsa_lcs_upload has not been called"); return FAMSA_E_STATE; }
+    FB_TRY(check_set(ctx, 1));
     if (!ctx->lcs.h_order.empty()) {
         set_error("famsa_dist_export: the set was uploaded with famsa_lcs_upload_sorted; the export works in the caller's order "
                   "(upload it with famsa_lcs_upload)");
@@ -592,9 +557,8 @@ int famsa_dist_export(famsa_ctx* ctx, int distance_kind, int square, int pid, co
     for (uint32_t i = 0; i < ctx->lcs.n; ++i)
         if (id_offsets[i + 1] < id_offsets[i]) { set_error("famsa_dist_export: id_offsets must not decrease"); return FAMSA_E_INVALID; }
     FB_CUDA(cudaSetDevice(ctx->device));
-    int rc = fb::scratch_acquire(ctx, ctx->stream);
-    if (rc) return rc;
-    rc = fb::dist_export(ctx, distance_kind, square, pid, ids, id_offsets, chunk_bytes, write, user, bytes_written);
+    FB_TRY(fb::scratch_acquire(ctx, ctx->stream));
+    const int rc = fb::dist_export(ctx, distance_kind, square, pid, ids, id_offsets, chunk_bytes, write, user, bytes_written);
     cudaStreamSynchronize(ctx->stream);
     fb::scratch_release(ctx, ctx->stream, true);
     return rc;
@@ -603,61 +567,39 @@ int famsa_dist_export(famsa_ctx* ctx, int distance_kind, int square, int pid, co
 int famsa_lcs_last_timing(const famsa_ctx* ctx, float* total_ms, float* main_kernel_ms, uint64_t* n_pairs)
 {
     FB_CHECK_CTX(ctx);
-    if (total_ms) *total_ms = ctx->lcs.last_total_ms;
-    if (main_kernel_ms) *main_kernel_ms = ctx->lcs.last_main_ms;
+    if (total_ms) *total_ms = ctx->lcs_timing.total_ms;
+    if (main_kernel_ms) *main_kernel_ms = ctx->lcs_timing.main_ms;
     if (n_pairs) *n_pairs = ctx->lcs.last_pairs;
     return FAMSA_OK;
 }
 
 // ------------------------------------------------------------------ HP-2
 
-static int dp_finish_timing(famsa_ctx* ctx)
-{
-    float total = 0.f, k = 0.f;
-    FB_CUDA(cudaEventSynchronize(ctx->ev[3]));
-    FB_CUDA(cudaEventElapsedTime(&total, ctx->ev[0], ctx->ev[3]));
-    FB_CUDA(cudaEventElapsedTime(&k, ctx->ev[1], ctx->ev[2]));
-    ctx->dp.last_total_ms = total;
-    ctx->dp.last_kernel_ms = k;
-    return FAMSA_OK;
-}
-
 int famsa_dp_align_batch(famsa_ctx* ctx, const famsa_dp_job* jobs, uint32_t n_jobs, const int64_t gaps[4],
                          famsa_dp_result* results, uint8_t* path_buf, uint8_t* dirs_buf)
 {
-    FB_CHECK_CTX(ctx);
-    if (n_jobs && (!jobs || !gaps || !results || !path_buf)) { set_error("NULL argument"); return FAMSA_E_INVALID; }
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    FB_CUDA(cudaSetDevice(ctx->device));
-    int rc = fb::scratch_acquire(ctx, ctx->stream);
-    if (rc) return rc;
-    rc = fb::dp_run_host(ctx, jobs, n_jobs, gaps, results, path_buf, dirs_buf);
-    if (rc) return rc;
-    fb::scratch_release(ctx, ctx->stream, true);
-    return dp_finish_timing(ctx);
+    return entry(ctx, nullptr, &famsa_ctx::dp_timing, [&]() -> int {
+        if (n_jobs && (!jobs || !gaps || !results || !path_buf)) { set_error("NULL argument"); return FAMSA_E_INVALID; }
+        return FAMSA_OK;
+    }, [&](cudaStream_t) { return fb::dp_run_host(ctx, jobs, n_jobs, gaps, results, path_buf, dirs_buf); });
 }
 
 int famsa_dp_align_batch_device(famsa_ctx* ctx, const famsa_dp_job* jobs, uint32_t n_jobs, const int64_t gaps[4],
                                 famsa_dp_result* d_results, uint8_t* d_path_buf, uint8_t* d_dirs_buf, void* stream)
 {
-    FB_CHECK_CTX(ctx);
-    if (n_jobs && (!jobs || !gaps || !d_results || !d_path_buf)) { set_error("NULL argument"); return FAMSA_E_INVALID; }
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    FB_CUDA(cudaSetDevice(ctx->device));
-    cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
-    int rc = fb::scratch_acquire(ctx, st);
-    if (rc) return rc;
-    rc = fb::dp_run_device(ctx, jobs, nullptr, n_jobs, gaps, d_results, d_path_buf, d_dirs_buf, nullptr, nullptr, st);
-    if (rc) return rc;
-    if (!stream) { FB_CUDA(cudaStreamSynchronize(st)); fb::scratch_release(ctx, st, true); return dp_finish_timing(ctx); }
-    return fb::scratch_release(ctx, st, false);
+    return entry(ctx, stream, &famsa_ctx::dp_timing, [&]() -> int {
+        if (n_jobs && (!jobs || !gaps || !d_results || !d_path_buf)) { set_error("NULL argument"); return FAMSA_E_INVALID; }
+        return FAMSA_OK;
+    }, [&](cudaStream_t st) {
+        return fb::dp_run_device(ctx, jobs, nullptr, n_jobs, gaps, d_results, d_path_buf, d_dirs_buf, nullptr, nullptr, st);
+    });
 }
 
 int famsa_dp_last_timing(const famsa_ctx* ctx, float* total_ms, float* kernel_ms, uint64_t* n_cells)
 {
     FB_CHECK_CTX(ctx);
-    if (total_ms) *total_ms = ctx->dp.last_total_ms;
-    if (kernel_ms) *kernel_ms = ctx->dp.last_kernel_ms;
+    if (total_ms) *total_ms = ctx->dp_timing.total_ms;
+    if (kernel_ms) *kernel_ms = ctx->dp_timing.main_ms;
     if (n_cells) *n_cells = ctx->dp.last_cells;
     return FAMSA_OK;
 }
@@ -685,30 +627,20 @@ int famsa_prof_put(famsa_ctx* ctx, const famsa_dp_profile* profiles, uint32_t n,
 int famsa_prof_merge_batch(famsa_ctx* ctx, const famsa_prof_merge* merges, uint32_t n, const int64_t gaps[4],
                            uint32_t* merged_ids_out, famsa_dp_result* results, uint8_t* path_buf, uint64_t path_cap)
 {
-    FB_CHECK_CTX(ctx);
-    if (n && (!merges || !gaps || !merged_ids_out || !results || !path_buf)) { set_error("NULL argument"); return FAMSA_E_INVALID; }
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    FB_CUDA(cudaSetDevice(ctx->device));
-    int rc = fb::scratch_acquire(ctx, ctx->stream);
-    if (rc) return rc;
-    rc = fb::prof_merge_batch(ctx, merges, n, gaps, merged_ids_out, results, path_buf, path_cap);
-    if (rc || !n) return rc;
-    return dp_finish_timing(ctx);
+    // an empty batch leaves the timing of the last one
+    return entry(ctx, nullptr, n ? &famsa_ctx::dp_timing : nullptr, [&]() -> int {
+        if (n && (!merges || !gaps || !merged_ids_out || !results || !path_buf)) { set_error("NULL argument"); return FAMSA_E_INVALID; }
+        return FAMSA_OK;
+    }, [&](cudaStream_t) { return fb::prof_merge_batch(ctx, merges, n, gaps, merged_ids_out, results, path_buf, path_cap); });
 }
 
 int famsa_prof_align_tree(famsa_ctx* ctx, const int32_t* tree, uint32_t n_leaves, const int64_t gaps[4],
                           famsa_dp_result* results, uint32_t* root_id_out, uint64_t* path_bytes_out, famsa_tree_stats* stats)
 {
-    FB_CHECK_CTX(ctx);
-    if (!tree || !gaps || !results) { set_error("NULL argument"); return FAMSA_E_INVALID; }
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    FB_CUDA(cudaSetDevice(ctx->device));
-    int rc = fb::scratch_acquire(ctx, ctx->stream);
-    if (rc) return rc;
-    rc = fb::prof_align_tree(ctx, tree, n_leaves, gaps, results, root_id_out, path_bytes_out, stats);
-    if (rc) return rc;
-    fb::scratch_release(ctx, ctx->stream, true);
-    return FAMSA_OK;
+    return entry(ctx, nullptr, nullptr, [&]() -> int {
+        if (!tree || !gaps || !results) { set_error("NULL argument"); return FAMSA_E_INVALID; }
+        return FAMSA_OK;
+    }, [&](cudaStream_t) { return fb::prof_align_tree(ctx, tree, n_leaves, gaps, results, root_id_out, path_bytes_out, stats); });
 }
 
 int famsa_prof_tree_paths(famsa_ctx* ctx, uint8_t* path_buf, uint64_t path_cap)

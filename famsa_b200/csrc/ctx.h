@@ -6,6 +6,7 @@
 #include <map>
 #include <mutex>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/famsa_b200.h"
@@ -26,13 +27,30 @@ const char* get_error();
         }                                                                                    \
     } while (0)
 
-// Simple owning device buffer that only grows.
+#define FB_TRY(expr)                       \
+    do {                                   \
+        int rc__ = (expr);                 \
+        if (rc__ != FAMSA_OK) return rc__; \
+    } while (0)
+
+// Owning device buffer that only grows; its memory goes with it.
 struct DevBuf {
     void* p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    DevBuf(DevBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); return *this; }   // o frees ours
+    ~DevBuf() { release(); }
     int reserve(size_t bytes);   // returns FAMSA_* code
     void release();
     template <class T> T* as() const { return static_cast<T*>(p); }
+};
+
+// Timing of the most recent call of a path, from the context's events: total = ev[0]..ev[3], main = ev[1]..ev[2]
+struct CallTiming {
+    float total_ms = 0.f, main_ms = 0.f;
 };
 
 // One 32-sequence mask group (sequences are grouped in length-descending order).
@@ -52,19 +70,26 @@ struct LcsState {
     std::vector<LcsGroupInfo> groups;
     std::vector<uint32_t> h_quirky;    // caller ids whose masks contain an all-ones 64-bit word
     std::vector<uint32_t> h_long;      // caller ids longer than the tile kernel handles as mask side
+    // element width that holds every LCS of the set: u16 while every sequence is shorter than 65536 residues
+    int elem_bytes() const { return max_len < 65536 ? 2 : 4; }
     DevBuf d_perm, d_invperm, d_len_sorted, d_code_off, d_codes, d_blob, d_group_blob;
-    DevBuf d_raw_codes, d_raw_off, d_raw_len, d_flags, d_pow075, d_assign_lcs, d_assign, d_mind,
-        d_pow075_f64, d_prim_tri, d_prim_side, d_prim_state, d_prim_out, d_prim_sideidx, d_prim_cand,
-        d_prim_dtri, d_prim_comp, d_prim_best, d_prim_part;
+    DevBuf d_raw_codes, d_raw_off, d_raw_len, d_flags, d_pow075, d_pow075_f64, d_assign_lcs, d_assign, d_mind;
+    // the guide trees and the export
+    DevBuf d_lcs_tri;                        // resident LCS triangle (prim, UPGMA, export), elem_bytes() wide
+    DevBuf d_dist_tri;                       // distance triangle: float64 for the Boruvka rounds, float32 for UPGMA
+    DevBuf d_side_idx, d_side_rows;          // lcs_side_rows: row of a flagged sequence in d_side_rows or -1; its u32 rows
+    DevBuf d_tree_state, d_tree_out, d_tree_cand;   // k_prim's or k_upgma's state, outputs and block candidates
+    DevBuf d_mst_comp, d_mst_best, d_mst_part;      // Boruvka rounds
     // per-call scratch
-    DevBuf d_tiles, d_res, d_refpos, d_ids_a, d_ids_b, d_out_stage, d_masks64, d_x64;
+    DevBuf d_tiles, d_res, d_refpos, d_ids_a, d_ids_b, d_out_stage, d_masks64, d_exact_rows, d_x64;
     // famsa_dist_export: per-sequence tables, the two device text chunks and their pinned host twins
-    DevBuf d_dx_meta, d_dx_ids, d_dx_side, d_dx_colq, d_dx_chunk[2];
+    DevBuf d_dx_meta, d_dx_ids, d_dx_colq, d_dx_chunk[2];
     char* h_dx_chunk[2] = {nullptr, nullptr};
     size_t h_dx_chunk_cap = 0;
     cudaEvent_t ev_dx[6] = {};               // per chunk buffer: format start, format end, copy done
-    // last-call timing
-    float last_total_ms = 0.f, last_main_ms = 0.f;
+    // last-call timing (famsa_ctx::lcs_timing): the entry point records ev[0] and ev[3]; lcs_triangle / lcs_rows mark
+    // their tile kernels in ev[1] and ev[2]
+    bool tiles_marked = false;               // ev[1] holds the first tile launch of the current call
     uint64_t last_pairs = 0;
     uint64_t last_tiles = 0;                 // tiles launched by the most recent triangle call
     std::vector<uint32_t> h_order;           // famsa_lcs_upload_sorted: position in the library's order -> caller index
@@ -75,7 +100,6 @@ struct DpState {
     void* h_pinned = nullptr;          // pinned staging buffer of the host entry point
     size_t h_pinned_cap = 0;
     uint64_t last_cells = 0;
-    float last_total_ms = 0.f, last_kernel_ms = 0.f;
 };
 
 // Profiles kept resident in HBM between the levels of the guide tree (prof.cu).
@@ -189,7 +213,7 @@ struct famsa_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
-    cudaStream_t copy_stream = nullptr;                 // D2H of finished row blocks (famsa_lcs_triangle)
+    cudaStream_t copy_stream = nullptr;                 // copies of finished pieces (triangle, exchange, export chunks)
     cudaEvent_t ev_block[8] = {};
     cudaEvent_t ev_copy[4] = {};                        // end of the peer copies of famsa_lcs_triangle_exchange, per copy stream
     cudaStream_t peer_stream[3] = {};                   // further copy streams: the peers of a piece are served side by side
@@ -207,6 +231,7 @@ struct famsa_ctx {
     int sm_count = 0;
     fb::LcsState lcs;
     fb::DpState dp;
+    fb::CallTiming lcs_timing, dp_timing;               // most recent call of each path (dp: main = the DP kernels)
     fb::ProfState prof;
 };
 
@@ -220,13 +245,20 @@ int lcs_upload(famsa_ctx* ctx, const int8_t* codes, const uint64_t* offsets, con
 int lcs_triangle(famsa_ctx* ctx, uint32_t row_begin, uint32_t row_end, void* d_out, int elem_bytes,
                  cudaStream_t stream, const uint32_t* bounds = nullptr, int n_blocks = 1,
                  cudaEvent_t* block_events = nullptr, bool quirk_fixups = true, bool piece_streams = false);
-int lcs_rows(famsa_ctx* ctx, const uint32_t* d_ref_ids, const uint32_t* h_ref_ids, uint32_t n_ref,
-             const uint32_t* d_col_ids, uint32_t n_col, void* d_out, int elem_bytes,
-             cudaStream_t stream, uint32_t g_begin = 0, uint32_t g_end = 0xffffffffu);
+// bounds[0..n_pieces] of the row range cut into pieces of equal pairs (frac: the cumulative share of each cut instead),
+// every inner cut on a mask-group boundary so that no group is computed twice
+void lcs_row_pieces(uint32_t row_begin, uint32_t row_end, int n_pieces, const double* frac, uint32_t* bounds);
+int lcs_rows(famsa_ctx* ctx, const uint32_t* h_ref_ids, uint32_t n_ref, const uint32_t* d_col_ids, uint32_t n_col, void* d_out,
+             int elem_bytes, cudaStream_t stream, uint32_t g_begin = 0, uint32_t g_end = 0xffffffffu);
+int lcs_side_rows(famsa_ctx* ctx, cudaStream_t st);
 int lcs_upgma(famsa_ctx* ctx, int kind, int modified, int32_t* h_tree, const void* d_tri_in = nullptr, int tri_eb = 2);
 int lcs_assign_shard(famsa_ctx* ctx, const uint32_t* h_seed_ids, uint32_t n_seeds, int kind, uint32_t shard, uint32_t n_shards,
                      long long* d_packed, cudaStream_t st);
-int lcs_prim(famsa_ctx* ctx, int kind, int32_t* h_from, int32_t* h_to, double* h_dist, int32_t* h_order);
+struct MstEdge { uint32_t a, b; double d; };
+// Boruvka rounds fill `tree` and leave the outputs to prim_replay (host only); the sequential loop fills them itself
+int lcs_prim(famsa_ctx* ctx, int kind, int32_t* h_from, int32_t* h_to, double* h_dist, int32_t* h_order,
+             std::vector<MstEdge>& tree);
+int prim_replay(const std::vector<MstEdge>& tree, int32_t* h_from, int32_t* h_to, double* h_dist, int32_t* h_order);
 int lcs_assign(famsa_ctx* ctx, const uint32_t* h_seed_ids, uint32_t n_seeds, int kind, uint32_t* h_assign,
                float* h_mind);
 int lcs_pow075_f64(famsa_ctx* ctx, cudaStream_t st);

@@ -7,7 +7,7 @@
 //   * LCS: the packed triangle of the caller's order, computed once by the tile kernel and kept in HBM (row = seq0, the
 //     dropped-carry rows already recomputed by the exact path).  Square mode reads the upper part from the mirror
 //     cell, which is only right when neither sequence is orientation dependent: rows of flagged sequences come from
-//     side rows (famsa_lcs_rows), columns of flagged sequences from an exact block (every row as seq0 against them), and
+//     side rows (lcs_side_rows), columns of flagged sequences from an exact block (every row as seq0 against them), and
 //     the diagonal of the others is the number of residues that can match (codes < 20).
 //   * Text: pass 1 sums every row's byte count (the width of a value depends on it alone); the host cuts the rows into
 //     chunks and prefix-sums the row offsets; pass 2, one block per row, formats 1024 values at a time: per-value
@@ -26,12 +26,6 @@
 #include "transform_dev.cuh"
 
 namespace fb {
-
-#define FB_TRY(expr)                      \
-    do {                                  \
-        int rc__ = (expr);                \
-        if (rc__ != FAMSA_OK) return rc__; \
-    } while (0)
 
 constexpr int kFmtThreads = 256;
 constexpr int kFmtPerThread = 4;                                  // consecutive columns per thread: contiguous text
@@ -252,7 +246,6 @@ static int nomem(famsa_ctx* ctx, const char* what, uint64_t bytes)
 void dist_export_release(famsa_ctx* ctx)
 {
     LcsState& S = ctx->lcs;
-    for (DevBuf* b : {&S.d_dx_meta, &S.d_dx_ids, &S.d_dx_side, &S.d_dx_colq, &S.d_dx_chunk[0], &S.d_dx_chunk[1]}) b->release();
     for (char*& h : S.h_dx_chunk)
         if (h) { cudaFreeHost(h); h = nullptr; }
     S.h_dx_chunk_cap = 0;
@@ -266,32 +259,29 @@ int dist_export(famsa_ctx* ctx, int kind, int square, int pid, const char* ids, 
     LcsState& S = ctx->lcs;
     cudaStream_t st = ctx->stream;
     const uint32_t n = S.n;
-    const int eb = S.max_len < 65536 ? 2 : 4;
+    const int eb = S.elem_bytes();
     const uint64_t pairs = (uint64_t)n * (n - 1) / 2;
     uint64_t written = 0;
     if (bytes_written) *bytes_written = 0;
     if (!S.ev_dx[0])
         for (int e = 0; e < 6; ++e) FB_CUDA(cudaEventCreateWithFlags(&S.ev_dx[e], e % 3 == 2 ? cudaEventDisableTiming : cudaEventDefault));
-    if (!ctx->copy_stream) {
-        FB_CUDA(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
-        for (auto& e : ctx->ev_block) FB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        for (auto& e : ctx->ev_host) FB_CUDA(cudaEventCreate(&e));
-    }
 
     // 1. the LCS triangle in caller order (row = seq0), resident for the whole call
-    if (S.d_prim_tri.reserve(std::max<uint64_t>(pairs, 1) * eb)) return nomem(ctx, "the LCS triangle", pairs * eb);
-    FB_TRY(lcs_triangle(ctx, 0, n, S.d_prim_tri.p, eb, st));
+    if (S.d_lcs_tri.reserve(std::max<uint64_t>(pairs, 1) * eb)) return nomem(ctx, "the LCS triangle", pairs * eb);
+    S.tiles_marked = false;
+    FB_CUDA(cudaEventRecord(ctx->ev[0], st));
+    FB_TRY(lcs_triangle(ctx, 0, n, S.d_lcs_tri.p, eb, st));
+    FB_CUDA(cudaEventRecord(ctx->ev[3], st));
     FB_CUDA(cudaStreamSynchronize(st));
     float lcs_total = 0.f, lcs_main = 0.f;
     FB_CUDA(cudaEventElapsedTime(&lcs_total, ctx->ev[0], ctx->ev[3]));
     FB_CUDA(cudaEventElapsedTime(&lcs_main, ctx->ev[1], ctx->ev[2]));
 
-    // 2. per-sequence tables: side index, diagonal, row byte counts and starts, id offsets
-    const size_t meta_bytes = sizeof(int) * n + sizeof(uint32_t) * n + sizeof(unsigned long long) * (3 * (size_t)n + 2);
+    // 2. per-sequence tables: diagonal, row byte counts and starts, id offsets
+    const size_t meta_bytes = sizeof(uint32_t) * n + sizeof(unsigned long long) * (3 * (size_t)n + 2);
     if (S.d_dx_meta.reserve(meta_bytes + 64)) return nomem(ctx, "the per-sequence tables", meta_bytes);
-    int* d_side_idx = S.d_dx_meta.as<int>();
-    uint32_t* d_diag = reinterpret_cast<uint32_t*>(d_side_idx + n);
-    unsigned long long* d_row_bytes = reinterpret_cast<unsigned long long*>(S.d_dx_meta.as<char>() + (((size_t)8 * n + 15) & ~(size_t)15));
+    uint32_t* d_diag = S.d_dx_meta.as<uint32_t>();
+    unsigned long long* d_row_bytes = reinterpret_cast<unsigned long long*>(S.d_dx_meta.as<char>() + (((size_t)4 * n + 15) & ~(size_t)15));
     unsigned long long* d_row_start = d_row_bytes + n;
     unsigned long long* d_id_off = d_row_start + n + 1;
     const uint64_t id_bytes = id_offsets[n] - id_offsets[0];
@@ -301,23 +291,19 @@ int dist_export(famsa_ctx* ctx, int kind, int square, int pid, const char* ids, 
     if (id_bytes) FB_CUDA(cudaMemcpyAsync(S.d_dx_ids.p, ids + id_offsets[0], id_bytes, cudaMemcpyHostToDevice, st));
     FB_CUDA(cudaMemcpyAsync(d_id_off, id_off.data(), sizeof(unsigned long long) * (n + 1), cudaMemcpyHostToDevice, st));
 
+    // square: rows of the flagged sequences (seq0 = the flagged one) and their columns (seq0 = every other sequence)
     const uint32_t nq = square ? (uint32_t)S.h_quirky.size() : 0;
-    std::vector<int> side_idx(n, -1);
-    for (uint32_t q = 0; q < nq; ++q) side_idx[S.h_quirky[q]] = (int)q;
-    FB_CUDA(cudaMemcpyAsync(d_side_idx, side_idx.data(), sizeof(int) * n, cudaMemcpyHostToDevice, st));
     FB_CUDA(cudaEventRecord(ctx->ev_host[0], st));
     if (square) {
         k_dist_diag<<<(n + 7) / 8, 256, 0, st>>>(S.d_raw_codes.as<int8_t>(), S.d_raw_off.as<uint64_t>(), S.d_raw_len.as<uint32_t>(), n, d_diag);
         FB_CUDA(cudaGetLastError());
         ctx->launches++;
+        FB_TRY(lcs_side_rows(ctx, st));
     }
     if (nq) {
-        // rows of the flagged sequences (seq0 = the flagged one) and their columns (seq0 = every other sequence)
-        if (S.d_dx_side.reserve(sizeof(uint32_t) * nq * (size_t)n)) return nomem(ctx, "the flagged rows", sizeof(uint32_t) * nq * (uint64_t)n);
         if (S.d_dx_colq.reserve(sizeof(uint32_t) * nq * (size_t)n)) return nomem(ctx, "the flagged columns", sizeof(uint32_t) * nq * (uint64_t)n);
         FB_TRY(S.d_ids_a.reserve(sizeof(uint32_t) * nq));
         FB_CUDA(cudaMemcpyAsync(S.d_ids_a.p, S.h_quirky.data(), sizeof(uint32_t) * nq, cudaMemcpyHostToDevice, st));
-        FB_TRY(lcs_rows(ctx, S.d_ids_a.as<uint32_t>(), S.h_quirky.data(), nq, nullptr, n, S.d_dx_side.p, 4, st));
         std::vector<uint32_t> all(n);
         for (uint32_t r = 0; r < n; ++r) all[r] = r;
         FB_TRY(lcs_exact_block(ctx, all, S.d_ids_a.as<uint32_t>(), nq, S.d_dx_colq.p, 4, st));
@@ -325,12 +311,12 @@ int dist_export(famsa_ctx* ctx, int kind, int square, int pid, const char* ids, 
     if (!pid) FB_TRY(lcs_pow075_f64(ctx, st));
 
     DistParams P{};
-    P.tri = S.d_prim_tri.p; P.eb = eb; P.n = n;
+    P.tri = S.d_lcs_tri.p; P.eb = eb; P.n = n;
     P.lens = S.d_raw_len.as<uint32_t>();
     P.pow075 = S.d_pow075_f64.as<double>();
     P.never = nextafter(DBL_MAX, 0.0);
     P.kind = kind; P.pid = pid; P.square = square;
-    P.side_idx = d_side_idx; P.side = S.d_dx_side.as<uint32_t>(); P.colq = S.d_dx_colq.as<uint32_t>(); P.nq = nq;
+    P.side_idx = S.d_side_idx.as<int>(); P.side = S.d_side_rows.as<uint32_t>(); P.colq = S.d_dx_colq.as<uint32_t>(); P.nq = nq;
     P.diag = d_diag;
     P.ids = S.d_dx_ids.as<char>(); P.id_off = d_id_off;
 
@@ -427,8 +413,8 @@ int dist_export(famsa_ctx* ctx, int kind, int square, int pid, const char* ids, 
     }
     FB_CUDA(cudaStreamSynchronize(ctx->copy_stream));
     if (bytes_written) *bytes_written = written;
-    S.last_total_ms = lcs_total + prep_ms + fmt_ms;
-    S.last_main_ms = lcs_main;
+    ctx->lcs_timing.total_ms = lcs_total + prep_ms + fmt_ms;
+    ctx->lcs_timing.main_ms = lcs_main;
     S.last_pairs = square ? (uint64_t)n * n : pairs;
     return FAMSA_OK;
 }

@@ -1332,12 +1332,6 @@ extern "C" int famsa_debug_fused_phases(double out_ns[8])
 // host side
 // ------------------------------------------------------------------------------------------------
 
-#define FB_TRY(expr)                      \
-    do {                                  \
-        int rc__ = (expr);                \
-        if (rc__ != FAMSA_OK) return rc__; \
-    } while (0)
-
 template <int NW, bool CLUSTERED>
 static int configure_fill(famsa_ctx* ctx)
 {

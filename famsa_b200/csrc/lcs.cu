@@ -949,12 +949,6 @@ void DevBuf::release()
     cap = 0;
 }
 
-#define FB_TRY(expr)                      \
-    do {                                  \
-        int rc__ = (expr);                \
-        if (rc__ != FAMSA_OK) return rc__; \
-    } while (0)
-
 template <int NL>
 static int launch_tile(famsa_ctx* ctx, const TileParams& P, uint32_t n_tiles, cudaStream_t st)
 {
@@ -1174,14 +1168,37 @@ static int exact_rows(famsa_ctx* ctx, const std::vector<ExactReq>& reqs, const u
     const uint32_t* d_group_nl = reinterpret_cast<const uint32_t*>(S.d_group_blob.as<uint64_t>() + S.n_groups);
     for (size_t b0 = 0; b0 < batch.size(); b0 += 65535) {            // gridDim.y limit
         const size_t nb = std::min<size_t>(65535, batch.size() - b0);
-        FB_TRY(S.d_masks64.reserve(sizeof(ExactRow) * nb));
-        FB_CUDA(cudaMemcpyAsync(S.d_masks64.p, batch.data() + b0, sizeof(ExactRow) * nb, cudaMemcpyHostToDevice, st));
+        FB_TRY(S.d_exact_rows.reserve(sizeof(ExactRow) * nb));
+        FB_CUDA(cudaMemcpyAsync(S.d_exact_rows.p, batch.data() + b0, sizeof(ExactRow) * nb, cudaMemcpyHostToDevice, st));
         k_lcs_exact_batch<<<dim3((max_cols + 127) / 128, (unsigned)nb), 128, 0, st>>>(
             S.d_codes.as<uint8_t>(), S.d_code_off.as<uint32_t>(), S.d_len_sorted.as<uint32_t>(), S.d_invperm.as<uint32_t>(),
-            S.d_masks64.as<ExactRow>(), d_col_ids, d_group_nl, d_out, elem_bytes);
+            S.d_exact_rows.as<ExactRow>(), d_col_ids, d_group_nl, d_out, elem_bytes);
         FB_CUDA(cudaGetLastError());
         ctx->launches++;
     }
+    return FAMSA_OK;
+}
+
+void lcs_row_pieces(uint32_t row_begin, uint32_t row_end, int n_pieces, const double* frac, uint32_t* bounds)
+{
+    auto tri = [](uint64_t r) { return r ? r * (r - 1) / 2 : 0; };
+    const uint64_t pairs = tri(row_end) - tri(row_begin);
+    bounds[0] = row_begin;
+    for (int b = 1; b < n_pieces; ++b) {
+        const double share = frac ? (double)pairs * frac[b] : (double)pairs * b / n_pieces;
+        uint32_t r = (uint32_t)((1.0 + std::sqrt(1.0 + 8.0 * ((double)tri(row_begin) + share))) / 2.0);
+        r = (r + 16) / 32 * 32;
+        bounds[b] = std::min(std::max(r, bounds[b - 1]), row_end);
+    }
+    bounds[n_pieces] = row_end;
+}
+
+// The span of the tile kernels within the entry point's call: ev[1] at the first tile launch, ev[2] after the last
+static int mark_tiles_begin(famsa_ctx* ctx, cudaStream_t st)
+{
+    if (ctx->lcs.tiles_marked) return FAMSA_OK;
+    FB_CUDA(cudaEventRecord(ctx->ev[1], st));
+    ctx->lcs.tiles_marked = true;
     return FAMSA_OK;
 }
 
@@ -1193,8 +1210,6 @@ int lcs_triangle(famsa_ctx* ctx, uint32_t row_begin, uint32_t row_end, void* d_o
 {
     LcsState& S = ctx->lcs;
     const uint32_t n = S.n;
-    S.last_pairs = (uint64_t)row_end * (row_end ? row_end - 1 : 0) / 2 - (uint64_t)row_begin * (row_begin ? row_begin - 1 : 0) / 2;
-    FB_CUDA(cudaEventRecord(ctx->ev[0], st));
     const uint32_t whole[2] = {row_begin, row_end};
     if (!bounds || !S.identity_perm) { bounds = whole; n_blocks = 1; }
 
@@ -1227,7 +1242,7 @@ int lcs_triangle(famsa_ctx* ctx, uint32_t row_begin, uint32_t row_end, void* d_o
     std::vector<uint32_t> special;      // rows the tile kernel may not answer for: dropped-carry and over-long rows
     if (quirk_fixups) std::set_union(S.h_quirky.begin(), S.h_quirky.end(), S.h_long.begin(), S.h_long.end(), std::back_inserter(special));
     else special = S.h_long;         // true LCS everywhere: only the rows the tile kernel cannot reach
-    FB_CUDA(cudaEventRecord(ctx->ev[1], st));
+    FB_TRY(mark_tiles_begin(ctx, st));
     // Blocks in one stream would each end with a partly filled last wave (half a wave of tiles per block boundary: 0.4 ms at
     // C2).  Issued round-robin on the auxiliary streams instead, the block scheduler fills the tail of block b with the first
     // tiles of block b+1 and the blocks still finish in order.  (The exact kernels share one scratch: single stream then.)
@@ -1266,20 +1281,15 @@ int lcs_triangle(famsa_ctx* ctx, uint32_t row_begin, uint32_t row_end, void* d_o
             FB_CUDA(cudaStreamWaitEvent(st, ctx->ev_join[a], 0));
         }
     FB_CUDA(cudaEventRecord(ctx->ev[2], st));
-    FB_CUDA(cudaEventRecord(ctx->ev[3], st));
     return FAMSA_OK;
 }
 
-int lcs_rows(famsa_ctx* ctx, const uint32_t* d_ref_ids, const uint32_t* h_ref_ids, uint32_t n_ref,
-             const uint32_t* d_col_ids, uint32_t n_col, void* d_out, int elem_bytes, cudaStream_t st,
-             uint32_t g_begin, uint32_t g_end)
+int lcs_rows(famsa_ctx* ctx, const uint32_t* h_ref_ids, uint32_t n_ref, const uint32_t* d_col_ids, uint32_t n_col, void* d_out,
+             int elem_bytes, cudaStream_t st, uint32_t g_begin, uint32_t g_end)
 {
     LcsState& S = ctx->lcs;
-    const uint32_t n = S.n;
-    S.last_pairs = (uint64_t)n_ref * n_col;
-    FB_CUDA(cudaEventRecord(ctx->ev[0], st));
     const uint32_t npad = S.n_groups * 32;
-    const int res_bytes = S.max_len < 65536 ? 2 : 4;
+    const int res_bytes = S.elem_bytes();
 
     // streamed side = the reference rows (true LCS is symmetric); mask side = every group
     std::vector<uint32_t> refpos(n_ref);
@@ -1311,7 +1321,7 @@ int lcs_rows(famsa_ctx* ctx, const uint32_t* d_ref_ids, const uint32_t* h_ref_id
     P.rows_mode = 1;
     P.refpos = S.d_refpos.as<uint32_t>();
     P.ld_res = npad;
-    FB_CUDA(cudaEventRecord(ctx->ev[1], st));
+    FB_TRY(mark_tiles_begin(ctx, st));
     at = 0;
     for (uint32_t nl = 1; nl <= (uint32_t)kMaxNL; ++nl) {
         auto& v = by_nl[nl];
@@ -1341,30 +1351,27 @@ int lcs_rows(famsa_ctx* ctx, const uint32_t* d_ref_ids, const uint32_t* h_ref_id
         }
         FB_TRY(exact_rows(ctx, reqs, d_col_ids, d_out, elem_bytes, st));
     }
-    (void)d_ref_ids;
-    (void)n;
-    FB_CUDA(cudaEventRecord(ctx->ev[3], st));
     return FAMSA_OK;
 }
 
-// Parallel MST + host replay of Prim's visiting order (see the kernels above).  Expects the true-LCS triangle in
-// d_prim_tri and the pow table in d_pow075_f64.
-static int prim_boruvka(famsa_ctx* ctx, int kind, int eb, int32_t* h_from, int32_t* h_to, double* h_dist, int32_t* h_order)
+// Parallel MST (see the kernels above) into `edges`; prim_replay then gives Prim's visiting order.  Expects the true-LCS
+// triangle in d_lcs_tri and the pow table in d_pow075_f64.
+static int prim_boruvka(famsa_ctx* ctx, int kind, int eb, std::vector<MstEdge>& edges)
 {
     LcsState& S = ctx->lcs;
     cudaStream_t st = ctx->stream;
     const uint32_t n = S.n;
     const size_t pairs = (size_t)n * (n - 1) / 2;
     const uint32_t n_chunks = (n + kMstChunk - 1) / kMstChunk;
-    FB_TRY(S.d_prim_dtri.reserve(pairs * sizeof(double)));
-    FB_TRY(S.d_prim_comp.reserve(sizeof(uint32_t) * n));
-    FB_TRY(S.d_prim_best.reserve(sizeof(EdgeMin) * n));
-    FB_TRY(S.d_prim_part.reserve(sizeof(EdgeMin) * (size_t)n_chunks * n));
-    double* d_dtri = S.d_prim_dtri.as<double>();
-    uint32_t* d_comp = S.d_prim_comp.as<uint32_t>();
-    EdgeMin* d_best = S.d_prim_best.as<EdgeMin>();
-    EdgeMin* d_part = S.d_prim_part.as<EdgeMin>();
-    k_mst_dist<<<n - 1, 256, 0, st>>>(S.d_prim_tri.p, eb, n, S.d_raw_len.as<uint32_t>(), S.d_pow075_f64.as<double>(), kind,
+    FB_TRY(S.d_dist_tri.reserve(pairs * sizeof(double)));
+    FB_TRY(S.d_mst_comp.reserve(sizeof(uint32_t) * n));
+    FB_TRY(S.d_mst_best.reserve(sizeof(EdgeMin) * n));
+    FB_TRY(S.d_mst_part.reserve(sizeof(EdgeMin) * (size_t)n_chunks * n));
+    double* d_dtri = S.d_dist_tri.as<double>();
+    uint32_t* d_comp = S.d_mst_comp.as<uint32_t>();
+    EdgeMin* d_best = S.d_mst_best.as<EdgeMin>();
+    EdgeMin* d_part = S.d_mst_part.as<EdgeMin>();
+    k_mst_dist<<<n - 1, 256, 0, st>>>(S.d_lcs_tri.p, eb, n, S.d_raw_len.as<uint32_t>(), S.d_pow075_f64.as<double>(), kind,
                                       nextafter(DBL_MAX, 0.0), d_dtri);
     FB_CUDA(cudaGetLastError());
     ctx->launches++;
@@ -1376,8 +1383,7 @@ static int prim_boruvka(famsa_ctx* ctx, int kind, int eb, int32_t* h_from, int32
         while (parent[x] != x) { parent[x] = parent[parent[x]]; x = parent[x]; }
         return x;
     };
-    struct HostEdge { uint32_t a, b; double d; };
-    std::vector<HostEdge> edges;
+    edges.clear();
     edges.reserve(n - 1);
     std::vector<EdgeMin> best(n), cbest(n);
     const double none = kEdgeNone;
@@ -1407,16 +1413,21 @@ static int prim_boruvka(famsa_ctx* ctx, int kind, int eb, int32_t* h_from, int32
             const uint32_t ra = find(a), rb = find(b);
             if (ra == rb) continue;                                 // both sides elected the same edge
             parent[ra] = rb;
-            edges.push_back(HostEdge{a, b, cbest[c].d});
+            edges.push_back(MstEdge{a, b, cbest[c].d});
             --n_comp;
         }
         if (n_comp == before) { set_error("famsa_lcs_prim: no progress in a Boruvka round"); return FAMSA_E_CUDA; }
         for (uint32_t v = 0; v < n; ++v) comp[v] = find(v);
     }
-    FB_CUDA(cudaEventRecord(ctx->ev[3], st));
-    // Prim's visiting order from vertex 0, replayed on the tree (MSTPrim.cpp:366-386 restricted to tree edges)
+    return FAMSA_OK;
+}
+
+// Prim's visiting order from vertex 0, replayed on the tree (MSTPrim.cpp:366-386 restricted to tree edges)
+int prim_replay(const std::vector<MstEdge>& edges, int32_t* h_from, int32_t* h_to, double* h_dist, int32_t* h_order)
+{
+    const uint32_t n = (uint32_t)edges.size() + 1;
     std::vector<std::vector<std::tuple<double, unsigned long long, uint32_t>>> adj(n);
-    for (const HostEdge& e : edges) {
+    for (const MstEdge& e : edges) {
         const unsigned long long lo = std::min(e.a, e.b), hi = std::max(e.a, e.b);
         const unsigned long long key = ~((lo << 32) + hi);
         adj[e.a].emplace_back(e.d, key, e.b);
@@ -1469,39 +1480,45 @@ int lcs_exact_block(famsa_ctx* ctx, const std::vector<uint32_t>& rows, const uin
     return exact_rows(ctx, reqs, d_col_ids, d_out, elem_bytes, st);
 }
 
-int lcs_prim(famsa_ctx* ctx, int kind, int32_t* h_from, int32_t* h_to, double* h_dist, int32_t* h_order)
+// The sequences whose LCS depends on which side is the row (the dropped-carry corner, h_quirky): d_side_idx[caller id] =
+// their row in d_side_rows or -1, and d_side_rows = their n_flagged x n rows (u32) with the flagged sequence as seq0
+int lcs_side_rows(famsa_ctx* ctx, cudaStream_t st)
+{
+    LcsState& S = ctx->lcs;
+    const uint32_t n = S.n, nq = (uint32_t)S.h_quirky.size();
+    std::vector<int> side_idx(n, -1);
+    for (uint32_t q = 0; q < nq; ++q) side_idx[S.h_quirky[q]] = (int)q;
+    FB_TRY(S.d_side_idx.reserve(sizeof(int) * n));
+    FB_CUDA(cudaMemcpyAsync(S.d_side_idx.p, side_idx.data(), sizeof(int) * n, cudaMemcpyHostToDevice, st));
+    FB_TRY(S.d_side_rows.reserve(std::max<size_t>((size_t)nq * n, 1) * sizeof(uint32_t)));
+    if (nq) FB_TRY(lcs_rows(ctx, S.h_quirky.data(), nq, nullptr, n, S.d_side_rows.p, 4, st));
+    return FAMSA_OK;
+}
+
+int lcs_prim(famsa_ctx* ctx, int kind, int32_t* h_from, int32_t* h_to, double* h_dist, int32_t* h_order,
+             std::vector<MstEdge>& tree)
 {
     LcsState& S = ctx->lcs;
     cudaStream_t st = ctx->stream;
     const uint32_t n = S.n;
-    const int eb = S.max_len < 65536 ? 2 : 4;
+    const int eb = S.elem_bytes();
     const size_t pairs = (size_t)n * (n - 1) / 2;
-    FB_TRY(S.d_prim_tri.reserve(std::max<size_t>(pairs, 1) * eb));
-    // the true-LCS triangle (orientation-free) ...
-    FB_TRY(lcs_triangle(ctx, 0, n, S.d_prim_tri.p, eb, st, nullptr, 1, nullptr, /*quirk_fixups=*/false));
-    // ... plus, for the few sequences whose LCS depends on which side is the row, their own rows
-    std::vector<int> side_idx(n, -1);
-    for (size_t q = 0; q < S.h_quirky.size(); ++q) side_idx[S.h_quirky[q]] = (int)q;
-    FB_TRY(S.d_prim_sideidx.reserve(sizeof(int) * n));
-    FB_CUDA(cudaMemcpyAsync(S.d_prim_sideidx.p, side_idx.data(), sizeof(int) * n, cudaMemcpyHostToDevice, st));
-    const uint32_t nq = (uint32_t)S.h_quirky.size();
-    FB_TRY(S.d_prim_side.reserve(std::max<size_t>((size_t)nq * n, 1) * sizeof(uint32_t)));
-    if (nq) {
-        FB_TRY(S.d_ids_a.reserve(sizeof(uint32_t) * nq));
-        FB_CUDA(cudaMemcpyAsync(S.d_ids_a.p, S.h_quirky.data(), sizeof(uint32_t) * nq, cudaMemcpyHostToDevice, st));
-        FB_TRY(lcs_rows(ctx, S.d_ids_a.as<uint32_t>(), S.h_quirky.data(), nq, nullptr, n, S.d_prim_side.p, 4, st));
-    }
+    FB_TRY(S.d_lcs_tri.reserve(std::max<size_t>(pairs, 1) * eb));
+    // the true-LCS triangle (orientation-free) plus the own rows of the flagged sequences
+    FB_TRY(lcs_triangle(ctx, 0, n, S.d_lcs_tri.p, eb, st, nullptr, 1, nullptr, /*quirk_fixups=*/false));
+    FB_TRY(lcs_side_rows(ctx, st));
     FB_TRY(lcs_pow075_f64(ctx, st));
     if (S.h_quirky.empty() && n >= 2 && !getenv("FAMSA_PRIM_SEQUENTIAL")) {
-        const int rc = prim_boruvka(ctx, kind, eb, h_from, h_to, h_dist, h_order);
+        const int rc = prim_boruvka(ctx, kind, eb, tree);
         if (rc != FAMSA_E_NOMEM) return rc;                         // no room for the float64 triangle: sequential loop
+        tree.clear();
         set_error("");                                              // the failed reservation is not this call's outcome
     }
-    FB_TRY(S.d_prim_state.reserve((sizeof(PrimState) + 1) * (size_t)n + 64));
-    FB_TRY(S.d_prim_out.reserve((sizeof(int) * 3 + sizeof(double)) * (size_t)n + 64));
-    PrimState* d_state = S.d_prim_state.as<PrimState>();
+    FB_TRY(S.d_tree_state.reserve((sizeof(PrimState) + 1) * (size_t)n + 64));
+    FB_TRY(S.d_tree_out.reserve((sizeof(int) * 3 + sizeof(double)) * (size_t)n + 64));
+    PrimState* d_state = S.d_tree_state.as<PrimState>();
     unsigned char* d_vis = reinterpret_cast<unsigned char*>(d_state + n);
-    double* d_dist = S.d_prim_out.as<double>();
+    double* d_dist = S.d_tree_out.as<double>();
     int* d_from = reinterpret_cast<int*>(d_dist + n);
     int* d_to = d_from + n;
     int* d_order = d_to + n;
@@ -1509,18 +1526,17 @@ int lcs_prim(famsa_ctx* ctx, int kind, int32_t* h_from, int32_t* h_to, double* h
         int per_sm = 0;
         FB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_prim, 1024, 0));
         const uint32_t nblk = std::max(1u, std::min((uint32_t)(ctx->sm_count * std::max(per_sm, 1)), (n + 1023) / 1024));
-        FB_TRY(S.d_prim_cand.reserve(sizeof(PrimCand) * 2 * nblk));
-        const void* a_tri = S.d_prim_tri.p; int a_eb = eb; uint32_t a_n = n;
+        FB_TRY(S.d_tree_cand.reserve(sizeof(PrimCand) * 2 * nblk));
+        const void* a_tri = S.d_lcs_tri.p; int a_eb = eb; uint32_t a_n = n;
         const uint32_t* a_len = S.d_raw_len.as<uint32_t>(); const double* a_pow = S.d_pow075_f64.as<double>();
         int a_kind = kind; double a_never = nextafter(DBL_MAX, 0.0);
-        const int* a_sidx = S.d_prim_sideidx.as<int>(); const uint32_t* a_side = S.d_prim_side.as<uint32_t>();
-        PrimCand* a_cand = S.d_prim_cand.as<PrimCand>();
+        const int* a_sidx = S.d_side_idx.as<int>(); const uint32_t* a_side = S.d_side_rows.as<uint32_t>();
+        PrimCand* a_cand = S.d_tree_cand.as<PrimCand>();
         void* args[] = {&a_tri, &a_eb, &a_n, &a_len, &a_pow, &a_kind, &a_never, &a_sidx, &a_side, &d_state, &d_vis,
                         &a_cand, &d_from, &d_to, &d_dist, &d_order};
         FB_CUDA(cudaLaunchCooperativeKernel((void*)k_prim, dim3(nblk), dim3(1024), args, 0, st));
     }
     ctx->launches++;
-    FB_CUDA(cudaEventRecord(ctx->ev[3], st));
     if (n > 1) {
         FB_CUDA(cudaMemcpyAsync(h_from, d_from, sizeof(int) * (n - 1), cudaMemcpyDeviceToHost, st));
         FB_CUDA(cudaMemcpyAsync(h_to, d_to, sizeof(int) * (n - 1), cudaMemcpyDeviceToHost, st));
@@ -1536,21 +1552,20 @@ int lcs_assign(famsa_ctx* ctx, const uint32_t* h_seed_ids, uint32_t n_seeds, int
     LcsState& S = ctx->lcs;
     cudaStream_t st = ctx->stream;
     const uint32_t n = S.n;
-    const int eb = S.max_len < 65536 ? 2 : 4;
+    const int eb = S.elem_bytes();
     FB_TRY(S.d_assign_lcs.reserve((size_t)eb * n * n_seeds));
     FB_TRY(S.d_assign.reserve(sizeof(uint32_t) * n));
     FB_TRY(S.d_mind.reserve(sizeof(float) * n));
     FB_TRY(S.d_ids_a.reserve(sizeof(uint32_t) * n_seeds));
     FB_CUDA(cudaMemcpyAsync(S.d_ids_a.p, h_seed_ids, sizeof(uint32_t) * n_seeds, cudaMemcpyHostToDevice, st));
     // seed k is the row (seq0) of its distance vector, every sequence a column: exactly famsa_lcs_rows
-    FB_TRY(lcs_rows(ctx, S.d_ids_a.as<uint32_t>(), h_seed_ids, n_seeds, nullptr, n, S.d_assign_lcs.p, eb, st));
+    FB_TRY(lcs_rows(ctx, h_seed_ids, n_seeds, nullptr, n, S.d_assign_lcs.p, eb, st));
     const float never = (float)nextafter((double)FLT_MAX, 0.0);
     k_assign<<<(n + 255) / 256, 256, 0, st>>>(S.d_assign_lcs.p, eb, n, n_seeds, S.d_ids_a.as<uint32_t>(),
                                              S.d_raw_len.as<uint32_t>(), S.d_pow075.as<float>(), kind, never,
                                              S.d_assign.as<uint32_t>(), S.d_mind.as<float>());
     FB_CUDA(cudaGetLastError());
     ctx->launches++;
-    FB_CUDA(cudaEventRecord(ctx->ev[3], st));
     FB_CUDA(cudaMemcpyAsync(h_assign, S.d_assign.p, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost, st));
     FB_CUDA(cudaMemcpyAsync(h_mind, S.d_mind.p, sizeof(float) * n, cudaMemcpyDeviceToHost, st));
     FB_CUDA(cudaStreamSynchronize(st));
@@ -1564,25 +1579,22 @@ int lcs_upgma(famsa_ctx* ctx, int kind, int modified, int32_t* h_tree, const voi
     LcsState& S = ctx->lcs;
     cudaStream_t st = ctx->stream;
     const uint32_t n = S.n;
-    const int eb = d_tri_in ? tri_eb : (S.max_len < 65536 ? 2 : 4);
+    const int eb = d_tri_in ? tri_eb : S.elem_bytes();
     const size_t pairs = (size_t)n * (n - 1) / 2;
     const void* d_tri = d_tri_in;
     if (!d_tri) {
-        FB_TRY(S.d_prim_tri.reserve(std::max<size_t>(pairs, 1) * eb));
-        FB_TRY(lcs_triangle(ctx, 0, n, S.d_prim_tri.p, eb, st));
-        d_tri = S.d_prim_tri.p;
-    } else {
-        S.last_pairs = 0;
-        FB_CUDA(cudaEventRecord(ctx->ev[0], st)); FB_CUDA(cudaEventRecord(ctx->ev[1], st)); FB_CUDA(cudaEventRecord(ctx->ev[2], st));
+        FB_TRY(S.d_lcs_tri.reserve(std::max<size_t>(pairs, 1) * eb));
+        FB_TRY(lcs_triangle(ctx, 0, n, S.d_lcs_tri.p, eb, st));
+        d_tri = S.d_lcs_tri.p;
     }
-    FB_TRY(S.d_prim_dtri.reserve(std::max<size_t>(pairs, 1) * sizeof(float)));
-    FB_TRY(S.d_prim_state.reserve((sizeof(float) + sizeof(uint32_t) + sizeof(int)) * (size_t)n + 64));
-    FB_TRY(S.d_prim_out.reserve(sizeof(int) * 2 * (size_t)n + 64));
-    float* d_dist = S.d_prim_dtri.as<float>();
-    float* d_mind = S.d_prim_state.as<float>();
+    FB_TRY(S.d_dist_tri.reserve(std::max<size_t>(pairs, 1) * sizeof(float)));
+    FB_TRY(S.d_tree_state.reserve((sizeof(float) + sizeof(uint32_t) + sizeof(int)) * (size_t)n + 64));
+    FB_TRY(S.d_tree_out.reserve(sizeof(int) * 2 * (size_t)n + 64));
+    float* d_dist = S.d_dist_tri.as<float>();
+    float* d_mind = S.d_tree_state.as<float>();
     uint32_t* d_nn = reinterpret_cast<uint32_t*>(d_mind + n);
     int* d_node = reinterpret_cast<int*>(d_nn + n);
-    int* d_tree = S.d_prim_out.as<int>();
+    int* d_tree = S.d_tree_out.as<int>();
     int* d_status = d_tree + 2 * (size_t)(n - 1);
     const float never = (float)nextafter((double)FLT_MAX, 0.0);
     k_upgma_dist<<<n - 1, 256, 0, st>>>(d_tri, eb, n, S.d_raw_len.as<uint32_t>(), S.d_pow075.as<float>(), kind, never, d_dist);
@@ -1595,14 +1607,13 @@ int lcs_upgma(famsa_ctx* ctx, int kind, int modified, int32_t* h_tree, const voi
         int per_sm = 0;
         FB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, 1024, 0));
         const uint32_t nblk = std::max(1u, std::min((uint32_t)(ctx->sm_count * std::max(per_sm, 1)), (n + 1023) / 1024));
-        FB_TRY(S.d_prim_cand.reserve(sizeof(unsigned long long) * 2 * nblk));
+        FB_TRY(S.d_tree_cand.reserve(sizeof(unsigned long long) * 2 * nblk));
         uint32_t a_n = n;
-        unsigned long long* a_cand = S.d_prim_cand.as<unsigned long long>();
+        unsigned long long* a_cand = S.d_tree_cand.as<unsigned long long>();
         void* args[] = {&d_dist, &a_n, &d_mind, &d_nn, &d_node, &a_cand, &d_tree, &d_status};
         FB_CUDA(cudaLaunchCooperativeKernel(fn, dim3(nblk), dim3(1024), args, 0, st));
         ctx->launches++;
     }
-    FB_CUDA(cudaEventRecord(ctx->ev[3], st));
     int status = 0;
     FB_CUDA(cudaMemcpyAsync(h_tree, d_tree, sizeof(int) * 2 * (size_t)(n - 1), cudaMemcpyDeviceToHost, st));
     FB_CUDA(cudaMemcpyAsync(&status, d_status, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1617,13 +1628,13 @@ int lcs_assign_shard(famsa_ctx* ctx, const uint32_t* h_seed_ids, uint32_t n_seed
 {
     LcsState& S = ctx->lcs;
     const uint32_t n = S.n;
-    const int eb = S.max_len < 65536 ? 2 : 4;
+    const int eb = S.elem_bytes();
     const uint32_t g_begin = (uint32_t)((unsigned long long)S.n_groups * shard / n_shards);
     const uint32_t g_end = (uint32_t)((unsigned long long)S.n_groups * (shard + 1) / n_shards);
     FB_TRY(S.d_assign_lcs.reserve((size_t)eb * n * n_seeds));
     FB_TRY(S.d_ids_a.reserve(sizeof(uint32_t) * n_seeds));
     FB_CUDA(cudaMemcpyAsync(S.d_ids_a.p, h_seed_ids, sizeof(uint32_t) * n_seeds, cudaMemcpyHostToDevice, st));
-    FB_TRY(lcs_rows(ctx, S.d_ids_a.as<uint32_t>(), h_seed_ids, n_seeds, nullptr, n, S.d_assign_lcs.p, eb, st, g_begin, g_end));
+    FB_TRY(lcs_rows(ctx, h_seed_ids, n_seeds, nullptr, n, S.d_assign_lcs.p, eb, st, g_begin, g_end));
     S.last_pairs = 0;
     for (uint32_t g = g_begin; g < g_end; ++g) S.last_pairs += (uint64_t)std::min(32u, n - g * 32) * n_seeds;
     const float never = (float)nextafter((double)FLT_MAX, 0.0);
@@ -1632,7 +1643,6 @@ int lcs_assign_shard(famsa_ctx* ctx, const uint32_t* h_seed_ids, uint32_t n_seed
                                                     S.d_invperm.as<uint32_t>(), g_begin, g_end, d_packed);
     FB_CUDA(cudaGetLastError());
     ctx->launches++;
-    FB_CUDA(cudaEventRecord(ctx->ev[3], st));
     return FAMSA_OK;
 }
 

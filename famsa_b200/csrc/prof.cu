@@ -34,12 +34,6 @@
 
 namespace fb {
 
-#define FB_TRY(expr)                      \
-    do {                                  \
-        int rc__ = (expr);                \
-        if (rc__ != FAMSA_OK) return rc__; \
-    } while (0)
-
 namespace {
 
 __global__ void __launch_bounds__(256) k_prof_leaf(const LeafDesc* __restrict__ leaves, const int8_t* __restrict__ codes,

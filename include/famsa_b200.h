@@ -214,7 +214,9 @@ double famsa_transform_f64(int kind, uint32_t lcs, uint32_t len1, uint32_t len2)
 float famsa_transform_f32(int kind, uint32_t lcs, uint32_t len1, uint32_t len2);
 
 /* Timing of the most recent LCS call on this context, measured with CUDA events on the stream the
- * kernels ran on: total = all kernels of the call, main = the lcs tile kernel(s) only. */
+ * kernels ran on: total = all kernels of the call, main = from its first lcs tile kernel to the end of
+ * its last (an empty span in a call without one), n_pairs = the pairs the call computes (the whole
+ * triangle for famsa_lcs_prim and famsa_lcs_upgma). */
 int famsa_lcs_last_timing(const famsa_ctx* ctx, float* total_ms, float* main_kernel_ms,
                           uint64_t* n_pairs);
 
