@@ -482,6 +482,24 @@ int famsa_lcs_prim(famsa_ctx* ctx, int distance_kind, int32_t* edge_from, int32_
     return fb::prim_replay(tree, edge_from, edge_to, edge_dist, prim_order);     // host only: outside the call's timing
 }
 
+int famsa_lcs_slink(famsa_ctx* ctx, int distance_kind, int32_t* tree)
+{
+    std::vector<fb::MstEdge> edges;
+    const int rc = entry(ctx, nullptr, &famsa_ctx::lcs_timing, [&]() -> int {
+        FB_TRY(check_set(ctx, 1));
+        if (!tree && ctx->lcs.n > 1) { set_error("NULL argument"); return FAMSA_E_INVALID; }
+        if (distance_kind != 0 && distance_kind != 1) { set_error("SingleLinkage is instantiated for distance_kind 0 and 1 only"); return FAMSA_E_INVALID; }
+        return FAMSA_OK;
+    }, [&](cudaStream_t st) -> int {
+        ctx->lcs.last_pairs = tri(ctx->lcs.n);
+        return lcs_timed(ctx, st, [&] { return fb::lcs_slink(ctx, distance_kind, edges); });
+    });
+    if (rc || edges.empty()) return rc;
+    const uint32_t n = (uint32_t)edges.size() + 1;
+    fb::slink_labels(std::move(edges), n, tree);                                // host only: outside the call's timing
+    return FAMSA_OK;
+}
+
 int famsa_lcs_assign(famsa_ctx* ctx, const uint32_t* seed_ids, uint32_t n_seeds, int distance_kind, uint32_t* assignments,
                      float* min_dist)
 {

@@ -259,6 +259,9 @@ struct MstEdge { uint32_t a, b; double d; };
 int lcs_prim(famsa_ctx* ctx, int kind, int32_t* h_from, int32_t* h_to, double* h_dist, int32_t* h_order,
              std::vector<MstEdge>& tree);
 int prim_replay(const std::vector<MstEdge>& tree, int32_t* h_from, int32_t* h_to, double* h_dist, int32_t* h_order);
+// SLINK's MST into `edges` (either engine); slink_labels (host only) turns it into the n-1 merges of SLINK's tree
+int lcs_slink(famsa_ctx* ctx, int kind, std::vector<MstEdge>& edges);
+void slink_labels(std::vector<MstEdge> edges, uint32_t n, int32_t* tree);
 int lcs_assign(famsa_ctx* ctx, const uint32_t* h_seed_ids, uint32_t n_seeds, int kind, uint32_t* h_assign,
                float* h_mind);
 int lcs_pow075_f64(famsa_ctx* ctx, cudaStream_t st);

@@ -521,6 +521,8 @@ struct PrimState {                 // per sequence: best known connection to the
 // blocks agree on the next vertex without a second barrier.  Candidate slots are double-buffered by step parity.
 // tri: true-LCS triangle in caller order; side rows hold the row-oriented values of the sequences whose LCS is
 // orientation dependent (dropped-carry corner): side_idx[v] = row in `side` or -1.
+// kSlink (famsa_lcs_slink): tri is the triangle SLINK reads (row = seq0, dropped-carry rows exact), every lookup reads
+// it (side_idx and side are not read), and there is no lower-bound skip -- SingleLinkage has none.
 struct PrimCand {
     double dist;
     unsigned long long key;
@@ -528,6 +530,7 @@ struct PrimCand {
     int pad;
 };
 
+template <bool kSlink>
 __global__ void __launch_bounds__(1024) k_prim(const void* __restrict__ tri, int eb, uint32_t n,
                                                const uint32_t* __restrict__ lens, const double* __restrict__ pow075,
                                                int kind, double never, const int* __restrict__ side_idx,
@@ -564,7 +567,7 @@ __global__ void __launch_bounds__(1024) k_prim(const void* __restrict__ tri, int
     grid.sync();
     for (uint32_t step = 1; step < n; ++step) {
         const uint32_t lv = lens[v];
-        const int sv = side_idx[v];
+        const int sv = kSlink ? -1 : side_idx[v];
         double bd = 0.0;
         unsigned long long bk = 0;
         int bid = -1;
@@ -579,7 +582,7 @@ __global__ void __launch_bounds__(1024) k_prim(const void* __restrict__ tri, int
         // reference's LCS can be larger, and then the skip decides whether the candidate is relaxed.
         if (has0 && !vis0) {
             const uint32_t j = gtid;
-            const bool tried = transform_f64(kind, lv < len0 ? lv : len0, lv, len0, pow075, never) <= d0;
+            const bool tried = kSlink || transform_f64(kind, lv < len0 ? lv : len0, lv, len0, pow075, never) <= d0;
             const double d = tried ? transform_f64(kind, lookup(j), lv, len0, pow075, never) : 1.7976931348623157e308;
             if (tried && d <= d0) {
                 const unsigned long long a = v < j ? v : j, b = v < j ? j : v;
@@ -593,7 +596,7 @@ __global__ void __launch_bounds__(1024) k_prim(const void* __restrict__ tri, int
             double cd = st[j].dist;
             unsigned long long ck = st[j].key;
             const uint32_t lj = lens[j];
-            const bool tried = transform_f64(kind, lv < lj ? lv : lj, lv, lj, pow075, never) <= cd;
+            const bool tried = kSlink || transform_f64(kind, lv < lj ? lv : lj, lv, lj, pow075, never) <= cd;
             const double d = tried ? transform_f64(kind, lookup(j), lv, lj, pow075, never) : 1.7976931348623157e308;
             if (tried && d <= cd) {
                 const unsigned long long a = v < j ? v : j, b = v < j ? j : v;
@@ -1495,6 +1498,43 @@ int lcs_side_rows(famsa_ctx* ctx, cudaStream_t st)
     return FAMSA_OK;
 }
 
+// The sequential vertex loop (k_prim) on d_lcs_tri, d_pow075_f64 and, for MSTPrim, the side rows.  Its outputs stay on
+// the device: edge k joins from[k] < to[k] at dist[k] and was added with the (k+1)-th vertex, order[i] = visiting position.
+struct PrimLoopOut {
+    double* dist;
+    int *from, *to, *order;
+};
+
+template <bool kSlink>
+static int prim_loop(famsa_ctx* ctx, int kind, int eb, cudaStream_t st, PrimLoopOut& o)
+{
+    LcsState& S = ctx->lcs;
+    const uint32_t n = S.n;
+    FB_TRY(S.d_tree_state.reserve((sizeof(PrimState) + 1) * (size_t)n + 64));
+    FB_TRY(S.d_tree_out.reserve((sizeof(int) * 3 + sizeof(double)) * (size_t)n + 64));
+    PrimState* d_state = S.d_tree_state.as<PrimState>();
+    unsigned char* d_vis = reinterpret_cast<unsigned char*>(d_state + n);
+    o.dist = S.d_tree_out.as<double>();
+    o.from = reinterpret_cast<int*>(o.dist + n);
+    o.to = o.from + n;
+    o.order = o.to + n;
+    int per_sm = 0;
+    FB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_prim<kSlink>, 1024, 0));
+    const uint32_t nblk = std::max(1u, std::min((uint32_t)(ctx->sm_count * std::max(per_sm, 1)), (n + 1023) / 1024));
+    FB_TRY(S.d_tree_cand.reserve(sizeof(PrimCand) * 2 * nblk));
+    const void* a_tri = S.d_lcs_tri.p; int a_eb = eb; uint32_t a_n = n;
+    const uint32_t* a_len = S.d_raw_len.as<uint32_t>(); const double* a_pow = S.d_pow075_f64.as<double>();
+    int a_kind = kind; double a_never = nextafter(DBL_MAX, 0.0);
+    const int* a_sidx = kSlink ? nullptr : S.d_side_idx.as<int>();
+    const uint32_t* a_side = kSlink ? nullptr : S.d_side_rows.as<uint32_t>();
+    PrimCand* a_cand = S.d_tree_cand.as<PrimCand>();
+    void* args[] = {&a_tri, &a_eb, &a_n, &a_len, &a_pow, &a_kind, &a_never, &a_sidx, &a_side, &d_state, &d_vis,
+                    &a_cand, &o.from, &o.to, &o.dist, &o.order};
+    FB_CUDA(cudaLaunchCooperativeKernel((void*)k_prim<kSlink>, dim3(nblk), dim3(1024), args, 0, st));
+    ctx->launches++;
+    return FAMSA_OK;
+}
+
 int lcs_prim(famsa_ctx* ctx, int kind, int32_t* h_from, int32_t* h_to, double* h_dist, int32_t* h_order,
              std::vector<MstEdge>& tree)
 {
@@ -1514,37 +1554,80 @@ int lcs_prim(famsa_ctx* ctx, int kind, int32_t* h_from, int32_t* h_to, double* h
         tree.clear();
         set_error("");                                              // the failed reservation is not this call's outcome
     }
-    FB_TRY(S.d_tree_state.reserve((sizeof(PrimState) + 1) * (size_t)n + 64));
-    FB_TRY(S.d_tree_out.reserve((sizeof(int) * 3 + sizeof(double)) * (size_t)n + 64));
-    PrimState* d_state = S.d_tree_state.as<PrimState>();
-    unsigned char* d_vis = reinterpret_cast<unsigned char*>(d_state + n);
-    double* d_dist = S.d_tree_out.as<double>();
-    int* d_from = reinterpret_cast<int*>(d_dist + n);
-    int* d_to = d_from + n;
-    int* d_order = d_to + n;
-    {
-        int per_sm = 0;
-        FB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_prim, 1024, 0));
-        const uint32_t nblk = std::max(1u, std::min((uint32_t)(ctx->sm_count * std::max(per_sm, 1)), (n + 1023) / 1024));
-        FB_TRY(S.d_tree_cand.reserve(sizeof(PrimCand) * 2 * nblk));
-        const void* a_tri = S.d_lcs_tri.p; int a_eb = eb; uint32_t a_n = n;
-        const uint32_t* a_len = S.d_raw_len.as<uint32_t>(); const double* a_pow = S.d_pow075_f64.as<double>();
-        int a_kind = kind; double a_never = nextafter(DBL_MAX, 0.0);
-        const int* a_sidx = S.d_side_idx.as<int>(); const uint32_t* a_side = S.d_side_rows.as<uint32_t>();
-        PrimCand* a_cand = S.d_tree_cand.as<PrimCand>();
-        void* args[] = {&a_tri, &a_eb, &a_n, &a_len, &a_pow, &a_kind, &a_never, &a_sidx, &a_side, &d_state, &d_vis,
-                        &a_cand, &d_from, &d_to, &d_dist, &d_order};
-        FB_CUDA(cudaLaunchCooperativeKernel((void*)k_prim, dim3(nblk), dim3(1024), args, 0, st));
-    }
-    ctx->launches++;
+    PrimLoopOut o;
+    FB_TRY(prim_loop<false>(ctx, kind, eb, st, o));
     if (n > 1) {
-        FB_CUDA(cudaMemcpyAsync(h_from, d_from, sizeof(int) * (n - 1), cudaMemcpyDeviceToHost, st));
-        FB_CUDA(cudaMemcpyAsync(h_to, d_to, sizeof(int) * (n - 1), cudaMemcpyDeviceToHost, st));
-        FB_CUDA(cudaMemcpyAsync(h_dist, d_dist, sizeof(double) * (n - 1), cudaMemcpyDeviceToHost, st));
+        FB_CUDA(cudaMemcpyAsync(h_from, o.from, sizeof(int) * (n - 1), cudaMemcpyDeviceToHost, st));
+        FB_CUDA(cudaMemcpyAsync(h_to, o.to, sizeof(int) * (n - 1), cudaMemcpyDeviceToHost, st));
+        FB_CUDA(cudaMemcpyAsync(h_dist, o.dist, sizeof(double) * (n - 1), cudaMemcpyDeviceToHost, st));
     }
-    FB_CUDA(cudaMemcpyAsync(h_order, d_order, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
+    FB_CUDA(cudaMemcpyAsync(h_order, o.order, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
     FB_CUDA(cudaStreamSynchronize(st));
     return FAMSA_OK;
+}
+
+// famsa_lcs_slink: SingleLinkage<>::run (SingleLinkage.cpp:30-189) orders distances by (distance, ids_to_uint64
+// descending), the strict order of the MST engines above, so its hierarchy is the unique MST merged in Kruskal order.
+// The triangle is the one SLINK reads (row i = seq0 against j < i, dropped-carry rows exact), so the distances are
+// symmetric and the Boruvka rounds serve whatever the set; the sequential loop runs when their float64 triangle does not
+// fit or FAMSA_PRIM_SEQUENTIAL is set.  `edges` gets the n-1 MST edges in no particular order; slink_labels names them.
+int lcs_slink(famsa_ctx* ctx, int kind, std::vector<MstEdge>& edges)
+{
+    LcsState& S = ctx->lcs;
+    cudaStream_t st = ctx->stream;
+    const uint32_t n = S.n;
+    const int eb = S.elem_bytes();
+    const size_t pairs = (size_t)n * (n - 1) / 2;
+    edges.clear();
+    if (n < 2) return FAMSA_OK;
+    FB_TRY(S.d_lcs_tri.reserve(pairs * eb));
+    FB_TRY(lcs_triangle(ctx, 0, n, S.d_lcs_tri.p, eb, st, nullptr, 1, nullptr, /*quirk_fixups=*/true));
+    FB_TRY(lcs_pow075_f64(ctx, st));
+    if (!getenv("FAMSA_PRIM_SEQUENTIAL")) {
+        const int rc = prim_boruvka(ctx, kind, eb, edges);
+        if (rc != FAMSA_E_NOMEM) return rc;                         // no room for the float64 triangle: sequential loop
+        edges.clear();
+        set_error("");                                              // the failed reservation is not this call's outcome
+    }
+    PrimLoopOut o;
+    FB_TRY(prim_loop<true>(ctx, kind, eb, st, o));
+    std::vector<int> from(n - 1), to(n - 1);
+    std::vector<double> dist(n - 1);
+    FB_CUDA(cudaMemcpyAsync(from.data(), o.from, sizeof(int) * (n - 1), cudaMemcpyDeviceToHost, st));
+    FB_CUDA(cudaMemcpyAsync(to.data(), o.to, sizeof(int) * (n - 1), cudaMemcpyDeviceToHost, st));
+    FB_CUDA(cudaMemcpyAsync(dist.data(), o.dist, sizeof(double) * (n - 1), cudaMemcpyDeviceToHost, st));
+    FB_CUDA(cudaStreamSynchronize(st));
+    edges.reserve(n - 1);
+    for (uint32_t k = 0; k + 1 < n; ++k) edges.push_back(MstEdge{(uint32_t)from[k], (uint32_t)to[k], dist[k]});
+    return FAMSA_OK;
+}
+
+// SLINK's tree from its MST (famsa_b200/mst.py slink_tree is the same in numpy): the edges in (distance, key) order; for
+// the edge joining clusters whose largest members are a < b, emit (node(a), node(b)) as merge k and key the merged
+// cluster, node n + k, by b.  This is what SLINK's stable_sort of lambda and its index relabelling produce (:166-188).
+void slink_labels(std::vector<MstEdge> edges, uint32_t n, int32_t* tree)
+{
+    auto key = [](const MstEdge& e) { return ~(((unsigned long long)std::min(e.a, e.b) << 32) + std::max(e.a, e.b)); };
+    std::sort(edges.begin(), edges.end(), [&](const MstEdge& x, const MstEdge& y) {
+        return x.d < y.d || (x.d == y.d && key(x) < key(y));
+    });
+    std::vector<uint32_t> parent(n), top(n), node(n);
+    std::iota(parent.begin(), parent.end(), 0u);
+    std::iota(top.begin(), top.end(), 0u);
+    std::iota(node.begin(), node.end(), 0u);
+    auto find = [&](uint32_t x) {
+        while (parent[x] != x) { parent[x] = parent[parent[x]]; x = parent[x]; }
+        return x;
+    };
+    for (size_t k = 0; k < edges.size(); ++k) {
+        const uint32_t ra = find(edges[k].a), rb = find(edges[k].b);
+        const uint32_t lo = std::min(top[ra], top[rb]), hi = std::max(top[ra], top[rb]);
+        tree[2 * k] = (int32_t)node[lo];
+        tree[2 * k + 1] = (int32_t)node[hi];
+        node[hi] = n + (uint32_t)k;
+        parent[ra] = rb;
+        top[rb] = hi;
+    }
 }
 
 int lcs_assign(famsa_ctx* ctx, const uint32_t* h_seed_ids, uint32_t n_seeds, int kind, uint32_t* h_assign, float* h_mind)

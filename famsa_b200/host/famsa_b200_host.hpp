@@ -12,6 +12,7 @@
 //   MSTPrim<>::run_view's vertex loop        src/tree/MSTPrim.cpp:280-549            CLCSBP::PrimEdges(...)
 //   CProfile(p1, p2) merge ctor, tables kept  profile.cpp:69-75, 784-1002            famsa_b200::ResidentProfiles
 //   DistanceCalculator<distance>::run        src/tree/DistanceCalculator.cpp:10-122   famsa_b200::ExportDistances(...)
+//   SingleLinkage<distance>::run             src/tree/SingleLinkage.cpp:30-189        famsa_b200::SingleLinkageTree(...)
 //     on the device between tree levels
 // Errors: the reference throws std::runtime_error and catches it in main() (src/famsa.cpp:160-165);
 // every non-zero C-ABI status is rethrown here the same way.  There is no CPU fallback.
@@ -287,6 +288,18 @@ inline std::vector<std::pair<int, int>> UPGMATree(Context& ctx, Distance measure
     if (measure == Distance::pairwise_identity) throw std::runtime_error("famsa_b200: UPGMA is instantiated for the two indel distances only");
     std::vector<int32_t> t(2 * (size_t)std::max<uint32_t>(n, 1));
     check(famsa_lcs_upgma(ctx.get(), measure == Distance::indel075_div_lcs ? 0 : 1, modified ? 1 : 0, t.data()));
+    std::vector<std::pair<int, int>> out;
+    for (uint32_t k = 0; k + 1 < n; ++k) out.emplace_back(t[2 * k], t[2 * k + 1]);
+    return out;
+}
+
+// SingleLinkage<distance>::run (SingleLinkage.cpp:30-189) on the device: the n - 1 merges, tree_structure's internal-node part
+inline std::vector<std::pair<int, int>> SingleLinkageTree(Context& ctx, Distance measure)
+{
+    const uint32_t n = famsa_lcs_n_seqs(ctx.get());
+    if (measure == Distance::pairwise_identity) throw std::runtime_error("famsa_b200: SingleLinkage is instantiated for the two indel distances only");
+    std::vector<int32_t> t(2 * (size_t)std::max<uint32_t>(n, 1));
+    check(famsa_lcs_slink(ctx.get(), measure == Distance::indel075_div_lcs ? 0 : 1, t.data()));
     std::vector<std::pair<int, int>> out;
     for (uint32_t k = 0; k + 1 < n; ++k) out.emplace_back(t[2 * k], t[2 * k + 1]);
     return out;

@@ -13,8 +13,8 @@ O(n log n).  Precondition: distances must not depend on which endpoint is the ro
 sequences of the reference's dropped-carry corner (64 identical residues on a word boundary); sets that contain such a
 sequence keep the sequential loop (famsa_lcs_prim).
 
-This module holds the two host pieces (edge order, Prim-order replay) and a reference Kruskal used by the tests; the
-device kernel is the next step (DESIGN.md section 6).
+This module holds the host pieces (edge order, Prim-order replay, SLINK's labelling of the same MST) and a reference
+Kruskal used by the tests; the device side is famsa_lcs_prim / famsa_lcs_slink (DESIGN.md section 6).
 """
 from __future__ import annotations
 
@@ -53,6 +53,34 @@ def kruskal_total_order(n: int, tri: np.ndarray) -> list[tuple[int, int, float]]
             out.append((a, b, float(tri[e])))
             if len(out) == n - 1:
                 break
+    return out
+
+
+def slink_tree(n: int, edges) -> np.ndarray:
+    """SingleLinkage<>::run's tree (SingleLinkage.cpp:30-189) from the MST of its distances.  With SLINK_HANDLE_TIES the
+    reference orders distances by (distance, ids_to_uint64 descending) -- the order above -- so its hierarchy is that
+    MST merged in Kruskal order, and its relabelling (stable_sort of lambda, then index[pi[j]] = n + k) names a merge
+    by the largest member of each side: for the edge joining clusters with largest members a < b, emit
+    (node(a), node(b)); the merged cluster becomes node n + k, keyed by b.  edges: n-1 (from, to, dist) in any order.
+    Returns the n-1 merges, (n-1, 2) int32.  famsa_b200/csrc/lcs.cu slink_labels is the same code in C++."""
+    order = sorted(edges, key=lambda e: (e[2], edge_key(e[0], e[1])))
+    parent = list(range(n))
+    top = list(range(n))                                # largest member of the cluster rooted here
+    node = list(range(n))                               # current node id of the cluster keyed by a member
+
+    def find(x):
+        while parent[x] != x:
+            parent[x] = parent[parent[x]]
+            x = parent[x]
+        return x
+    out = np.zeros((max(n - 1, 0), 2), dtype=np.int32)
+    for k, (a, b, _) in enumerate(order):
+        ra, rb = find(int(a)), find(int(b))
+        lo, hi = sorted((top[ra], top[rb]))
+        out[k] = node[lo], node[hi]
+        node[hi] = n + k
+        parent[ra] = rb
+        top[rb] = hi
     return out
 
 

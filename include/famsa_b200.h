@@ -184,6 +184,21 @@ int famsa_lcs_upgma(famsa_ctx* ctx, int distance_kind, int modified, int32_t* tr
 int famsa_lcs_upgma_from_triangle(famsa_ctx* ctx, int distance_kind, int modified, const void* d_triangle, int elem_bytes,
                                   int32_t* tree);
 
+/* The single-linkage guide tree (-gt slink): SingleLinkage<distance>::run (src/tree/SingleLinkage.cpp:30-189) on the
+ * device.  SLINK reads row i (sequence i as the row, seq0) against 0..i-1 through Transform<double, distance> and, with
+ * SLINK_HANDLE_TIES (SingleLinkage.h:16-38), orders distances by (distance ascending, ids_to_uint64 descending): the
+ * strict total order famsa_lcs_prim uses.  Under a strict order the single-linkage hierarchy is the unique minimum
+ * spanning tree merged in Kruskal order, and SLINK's output (stable_sort of lambda, then index[pi[j]] = n + k, :166-188)
+ * names each merge by the largest member of its two sides.  So the library finds that MST on the LCS triangle kept in
+ * HBM -- with the Boruvka rounds over a float64 distance triangle when it fits beside the LCS triangle, else with the
+ * sequential vertex loop (also when FAMSA_PRIM_SEQUENTIAL is set; without MSTPrim's lower-bound skip, which SLINK does
+ * not have) -- and labels it on the host.  Only the n-1 merges leave the device.  tree[2k], tree[2k+1] = children of
+ * internal node n_seqs + k, leaves 0..n-1 in caller order, which must be FAMSA's length-descending order
+ * (src/msa.cpp:245-256) for the reference's tree; the result is that tree pair for pair.  n_seqs = 1 gives no merges
+ * (tree may then be NULL).  distance_kind 0 (indel075_div_lcs) or 1 (indel_div_lcs), the two SingleLinkage
+ * instantiations.  famsa_lcs_last_timing: n_pairs = the whole triangle.  HOST pointer. */
+int famsa_lcs_slink(famsa_ctx* ctx, int distance_kind, int32_t* tree);
+
 /* The distance-matrix export (-dist_export [-square_matrix] [-pid]): DistanceCalculator<distance>::run
  * (src/tree/DistanceCalculator.cpp:10-122) with its text formatting, num2str / NumericConversions::Double2PChar
  * (src/utils/conversion.h:52-119), on the device.  Works on the set of the last famsa_lcs_upload, in the caller's
