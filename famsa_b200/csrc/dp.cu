@@ -236,14 +236,15 @@ __device__ __forceinline__ void prep_body(const DpParams& P, uint32_t jid)
     // variant and orientation (CProfile::Align, profile.cpp:254-304).  Everything the decision and the fill's choice of
     // arithmetic need is gathered in ONE pass over the tables and one reduction: per side the number of non-zero counters
     // (orientation of ProfProf), the largest |score| that can enter T and whether it leaves int32, and -- ProfProf only --
-    // whether every count the cell loop multiplies with is >= 0 (see ulo32).
+    // whether every count the cell loop multiplies with is >= 0 (see ulo32) and the largest sum of a column's counters
+    // over the symbols that enter T.
     int var, sw = 0;
     if (J.card1 == 1 && J.card2 == 1) var = 0;
     else if (J.card1 == 1) var = 1;
     else if (J.card2 == 1) { var = 1; sw = 1; }
     else var = 2;
-    __shared__ unsigned long long sm_red[2][3];                      // per side: nz, smax, flags (1 wide, 2 bad)
-    if (tid < 6) sm_red[tid / 3][tid % 3] = 0;
+    __shared__ unsigned long long sm_red[2][4];                      // per side: nz, smax, flags (1 wide, 2 bad), max column sum
+    if (tid < 8) sm_red[tid / 4][tid % 4] = 0;
     __syncthreads();
     for (int side = 0; side < 2; ++side) {
         const bool is_col = var == 2 || (side == 1) != (sw == 1);    // Seq*: only the column side's scores matter
@@ -251,7 +252,7 @@ __device__ __forceinline__ void prep_body(const DpParams& P, uint32_t jid)
         const int* cnt = side ? J.c2 : J.c1;
         const uint32_t w = side ? w2 : w1;
         const int card = (int)(side ? J.card2 : J.card1);
-        unsigned long long nz = 0, smax = 0, flags = 0;
+        unsigned long long nz = 0, smax = 0, flags = 0, csum_max = 0;
         // one thread per column, all loads of a column issued together (the block is small: memory-level parallelism
         // is what makes this pass short)
         for (uint32_t c = tid; c <= w; c += nthr) {
@@ -261,6 +262,7 @@ __device__ __forceinline__ void prep_body(const DpParams& P, uint32_t jid)
 #pragma unroll
                 for (int q = 0; q < 8; ++q) v[q] = cc[q];
                 int neg = 0, over = 0;
+                long long csum = 0;
 #pragma unroll
                 for (int q = 0; q < 8; ++q) {
                     nz += (v[q].x != 0) + (v[q].y != 0) + (v[q].z != 0) + (v[q].w != 0);
@@ -268,8 +270,11 @@ __device__ __forceinline__ void prep_body(const DpParams& P, uint32_t jid)
                     if (q == 7) { u.z = 0; u.w = 0; }                 // rows 30 (GAP) and 31 (GUARD) are not counts of a symbol
                     neg |= u.x | u.y | u.z | u.w;
                     over |= (u.x > card) | (u.y > card) | (u.z > card) | (u.w > card);
+                    csum += (long long)u.x + u.y + u.z + u.w;
                 }
                 if (c >= 1) {
+                    // (a negative counter makes the job bad, so the sum only matters when every term is >= 0)
+                    csum_max = csum > (long long)csum_max ? (unsigned long long)csum : csum_max;
                     int a2, b2, d2, e2, f2, g2;
                     solve_gaps(cnt, c, w, card, a2, b2, d2, e2, f2, g2);
                     if ((a2 | b2 | d2 | e2 | f2 | g2) < 0 || neg < 0 || over) flags |= 2;
@@ -295,11 +300,14 @@ __device__ __forceinline__ void prep_body(const DpParams& P, uint32_t jid)
             const unsigned long long x = __shfl_xor_sync(0xffffffffu, smax, o);
             smax = x > smax ? x : smax;
             flags |= __shfl_xor_sync(0xffffffffu, flags, o);
+            const unsigned long long y = __shfl_xor_sync(0xffffffffu, csum_max, o);
+            csum_max = y > csum_max ? y : csum_max;
         }
         if ((tid & 31) == 0) {
             if (nz) atomicAdd(&sm_red[side][0], nz);
             if (smax) atomicMax(&sm_red[side][1], smax);
             if (flags) atomicOr(&sm_red[side][2], flags);
+            if (csum_max) atomicMax(&sm_red[side][3], csum_max);
         }
     }
     __syncthreads();
@@ -316,9 +324,12 @@ __device__ __forceinline__ void prep_body(const DpParams& P, uint32_t jid)
         m.SR = SR; m.CR = CR; m.SC = SC; m.CC = CC; m.WR = WR; m.WC = WC; m.nR = nR; m.nC = nC; m.var = var; m.sw = sw;
         m.bad = var == 2 && ((sm_red[0][2] | sm_red[1][2]) & 2) ? 1 : 0;
         // column-pair scores: IMMA byte-digit planes need 32-bit scores and counters of one (card <= 127) or two
-        // (<= 32767) byte digits; |T| <= max|score| * (sum of the row's counters <= 7 * card) decides the ring's width
+        // (<= 32767) byte digits.  |T| <= max|score| * (largest sum of a row column's counters over symbols 0..29) decides
+        // the ring's width: 4 bytes when that sum is at most 7 * card (every profile CProfile builds has at most card) and
+        // max|score| < 2^31 / (7 * card); a table with a larger sum (which the checks above let through) gets 8 bytes.
         m.tmode = var != 2 ? 2 : (wide ? 2 : (nR <= 127 ? 0 : (nR <= 32767 ? 1 : 2)));
-        m.t32 = var == 2 ? smax < (1ull << 31) / (7ull * (unsigned long long)nR) : smax < (1ull << 31);
+        m.t32 = var == 2 ? smax < (1ull << 31) / (7ull * (unsigned long long)nR) && sm_red[1 - cs][3] <= 7ull * (unsigned long long)nR
+                         : smax < (1ull << 31);
         P.meta[jid] = m;
     }
     const Scratch L(J.w1, J.w2);
@@ -1721,7 +1732,7 @@ int dp_run_device(famsa_ctx* ctx, const famsa_dp_job* jobs, const DpJobExt* ext,
         ctx->launches += 1;
         // one launch per run of equal class in `order`; different classes run side by side (fork after prep, join before
         // the traceback) so that a level pays for its slowest merge once, not once per launch shape
-        static const bool debug = getenv("FAMSA_DP_DEBUG") != nullptr;
+        const bool debug = getenv("FAMSA_DP_DEBUG") != nullptr;       // development aid: one line per launch class
         uint32_t n_classes = 0;
         for (uint32_t q0 = 0; q0 < m;) { const int c = cls(order[q0]); while (q0 < m && cls(order[q0]) == c) ++q0; ++n_classes; }
         if (n_classes > 1) FB_CUDA(cudaEventRecord(ctx->ev_fork, st));
@@ -1731,8 +1742,9 @@ int dp_run_device(famsa_ctx* ctx, const famsa_dp_job* jobs, const DpJobExt* ext,
             const int c = cls(order[q0]);
             uint32_t q1 = q0;
             while (q1 < m && cls(order[q1]) == c) ++q1;
-            if (debug) fprintf(stderr, "[dp] batch of %u: class %d x %u (first %u x %u, %u stripes), demand %llu, cl_cap %u, latency_mode %d\n", m, c, q1 - q0,
+            if (debug) fprintf(stderr, "[dp] batch of %u: class %d x %u (first %u x %u, %u stripes), demand %llu, cl_cap %u, latency_mode %d", m, c, q1 - q0,
                                dev[order[q0]].w1, dev[order[q0]].w2, stripes_of(order[q0]), demand, cl_cap, (int)small_batch);
+            if (debug && c != 1) fprintf(stderr, "\n");                  // class 1 finishes the line with its team shape below
             DpParams Q = P;
             Q.order = P.order + q0;
             Q.n_jobs = q1 - q0;
@@ -1772,6 +1784,7 @@ int dp_run_device(famsa_ctx* ctx, const famsa_dp_job* jobs, const DpJobExt* ext,
                 else if (Q.n_jobs >= 4u * sms) nw = 2;
                 else if (Q.n_jobs >= 2u * sms) nw = 4;
                 if (nw_forced) { nw = nw_forced; compact = compact && (nw == 2 || nw == 4 || nw == 6); }
+                if (debug) fprintf(stderr, ", team %d, compact %d\n", nw == 2 || nw == 4 ? nw : (compact ? 6 : kDpTeamWarps), (int)compact);
                 if (compact) {
                     switch (nw) {
                     case 2: k_dp_fill_compact<2><<<Q.n_jobs, 2 * 32, 2 * kCompactStride, st>>>(Q); break;
