@@ -95,11 +95,24 @@ struct LcsState {
     std::vector<uint32_t> h_order;           // famsa_lcs_upload_sorted: position in the library's order -> caller index
 };
 
+// Sections of one allocation, each on a 256-byte boundary: add() returns a section's offset, `end` is the total size.
+struct Layout {
+    unsigned long long end = 0;
+    unsigned long long add(unsigned long long bytes)
+    {
+        const unsigned long long at = align_up(end, 256);
+        end = at + bytes;
+        return at;
+    }
+};
+
 struct DpState {
     DevBuf d_dirs_out, d_tables, d_results, d_path;     // host entry point only; per-call scratch is stream-ordered
     void* h_pinned = nullptr;          // pinned staging buffer of the host entry point
     size_t h_pinned_cap = 0;
     uint64_t last_cells = 0;
+    bool configured = false;           // the DP kernels' attributes are set and the cluster caps probed (dp.cu dp_setup)
+    uint32_t cl_cap = 0, duo_cap = 0;  // largest cluster of 4-warp k_dp_fill blocks / of k_dp_fill_duo blocks
 };
 
 // Profiles kept resident in HBM between the levels of the guide tree (prof.cu).
@@ -276,11 +289,10 @@ int dp_run_host(famsa_ctx* ctx, const famsa_dp_job* jobs, uint32_t n, const int6
                 uint8_t* path_buf, uint8_t* dirs_buf);
 int dp_check_results(const famsa_dp_result* results, uint32_t n);
 // d_meta_out / d_blob_out non-NULL: the per-job DpMeta records stay valid until the caller cudaFreeAsync()s *d_blob_out
-// fused non-NULL (a FusedParams, prof_dev.cuh): every merge runs whole -- leaves, prep, fill, traceback, merged tables --
-// in one block of k_merge_fused; the caller then launches neither the leaf nor the construct kernel.
 int dp_run_device(famsa_ctx* ctx, const famsa_dp_job* jobs, const DpJobExt* ext, uint32_t n, const int64_t gaps[4],
                   famsa_dp_result* d_results, uint8_t* d_path, uint8_t* d_dirs, DpMeta** d_meta_out, void** d_blob_out,
-                  cudaStream_t st, const void* fused = nullptr);
+                  cudaStream_t st);
+// out NULL: only the sizes of the plan
 int dp_fused_plan(const famsa_dp_job* jobs, const DpJobExt* ext, uint32_t n, bool align16, DpJobDev* out, DpFusedPlan* plan);
 int dp_fused_launch(famsa_ctx* ctx, const DpJobDev* jobs, uint32_t n, const int64_t gaps[4], famsa_dp_result* d_results, uint8_t* d_path,
                     DpMeta* d_meta, uint8_t* d_scratch, uint8_t* d_skew, famsa_dp_result* h_results, uint8_t* h_path,

@@ -27,27 +27,22 @@
 //              per step).  The same kernel then walks the direction matrix back and emits the path.
 //   k_dp_unskew only when the caller asks for CDPMatrix bytes: skewed directions -> row-major.
 #include <algorithm>
-#include <atomic>
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
-#include <numeric>
 #include <thread>
 
 #include <cooperative_groups.h>
 
 #include "ctx.h"
 #include "dp_dev.h"
+#include "dp_plan.h"
 #include "prof_dev.cuh"
 
 namespace fb {
 
 constexpr int kDpWarps = 4;               // warps (= merges) per block of the one-warp-per-merge fill kernel
 constexpr int kDpTeamWarps = 8;           // warps cooperating on one large merge
-constexpr uint32_t kDpTeamMinWidth = 96;  // min(w1, w2) above which a merge gets a team
 constexpr int kDpCluster = 8;             // thread blocks per cluster for the widest merges
-constexpr uint32_t kDpClusterMinWidth = 1024;   // min(w1, w2) above which a merge gets a whole cluster
-constexpr int kTThreads = 256, kTCellsPerThread = 4;
 
 // per column j of the column profile, 64 bytes, meaning depends on the variant:
 //   ProfProf: gap scores {S[j][GO], S[j][GE], S[j][TO], S[j][TE]}, chg, b0 = (s_o, s_e), b1 = (s_to, s_te), b2 = (k_e, k_te)
@@ -1343,112 +1338,114 @@ extern "C" int famsa_debug_fused_phases(double out_ns[8])
 // host side
 // ------------------------------------------------------------------------------------------------
 
-template <int NW, bool CLUSTERED>
-static int configure_fill(famsa_ctx* ctx)
+using DpKernelFn = void (*)(DpParams);
+
+// the instantiation that runs a fill launch
+static DpKernelFn fill_kernel(const DpLaunch& L)
 {
-    static std::atomic<bool> configured[64];
-    constexpr int warps = NW == 1 ? kDpWarps : NW;
-    if (!configured[ctx->device & 63].load(std::memory_order_acquire)) {
-        FB_CUDA(cudaFuncSetAttribute(k_dp_fill<NW, CLUSTERED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(warps * sizeof(WarpShared))));
-        if (CLUSTERED) FB_CUDA(cudaFuncSetAttribute(k_dp_fill<NW, CLUSTERED>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-        configured[ctx->device & 63].store(true, std::memory_order_release);
+    switch (L.kernel) {
+    case DpKernel::Duo: return k_dp_fill_duo;
+    case DpKernel::Compact: return L.nw == 2 ? k_dp_fill_compact<2> : (L.nw == 4 ? k_dp_fill_compact<4> : k_dp_fill_compact<6>);
+    default:
+        if (L.cluster > 1) return L.nw == 4 ? k_dp_fill<4, true> : k_dp_fill<kDpTeamWarps, true>;
+        return L.nw == 1 ? k_dp_fill<1, false> : (L.nw == 2 ? k_dp_fill<2, false> : (L.nw == 4 ? k_dp_fill<4, false> : k_dp_fill<kDpTeamWarps, false>));
     }
+}
+
+static bool clustered(const DpLaunch& L) { return L.kernel == DpKernel::Duo || L.cluster > 1; }
+
+// grid, block, dynamic shared memory and cluster size of a fill launch of n merges (attr: storage of the cluster attribute)
+static cudaLaunchConfig_t fill_config(const DpLaunch& L, uint32_t n, cudaStream_t st, cudaLaunchAttribute* attr)
+{
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(L.nw == 1 ? (n + kDpWarps - 1) / kDpWarps : n * L.cluster);
+    cfg.blockDim = dim3((L.nw == 1 ? kDpWarps : L.nw) * 32);
+    cfg.dynamicSmemBytes = L.kernel == DpKernel::Duo ? kDuoSmem
+                         : L.kernel == DpKernel::Compact ? L.nw * kCompactStride : (L.nw == 1 ? kDpWarps : L.nw) * sizeof(WarpShared);
+    cfg.stream = st;
+    attr->id = cudaLaunchAttributeClusterDimension;
+    attr->val.clusterDim.x = L.cluster;
+    attr->val.clusterDim.y = 1;
+    attr->val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = clustered(L) ? 1 : 0;
+    return cfg;
+}
+
+// the largest of `sizes` (ascending) up to the first cluster size the device refuses for L's kernel; `v` if none fits
+static uint32_t probe_cluster(DpLaunch L, uint32_t v, std::initializer_list<uint32_t> sizes)
+{
+    for (uint32_t cl : sizes) {
+        L.cluster = cl;
+        cudaLaunchAttribute attr;
+        const cudaLaunchConfig_t cfg = fill_config(L, 1, nullptr, &attr);
+        int n = 0;
+        if (cudaOccupancyMaxActiveClusters(&n, fill_kernel(L), &cfg) != cudaSuccess || n == 0) { cudaGetLastError(); break; }
+        v = cl;
+    }
+    return v;
+}
+
+// Once per context: every DP kernel's dynamic shared memory and cluster attributes, and the largest clusters the device
+// runs of the 4-warp fill kernel and of the producer / consumer kernel.
+static int dp_setup(famsa_ctx* ctx)
+{
+    DpState& S = ctx->dp;
+    if (S.configured) return FAMSA_OK;
+    const DpLaunch kernels[] = {{0, DpKernel::Fill, 1, 1},    {0, DpKernel::Fill, 2, 1},          {0, DpKernel::Fill, 4, 1},
+                                {0, DpKernel::Fill, kDpTeamWarps, 1}, {0, DpKernel::Fill, 4, 2}, {0, DpKernel::Fill, kDpTeamWarps, kDpCluster},
+                                {0, DpKernel::Compact, 2, 1}, {0, DpKernel::Compact, 4, 1},       {0, DpKernel::Compact, 6, 1},
+                                {0, DpKernel::Duo, 8, 2}};
+    for (const DpLaunch& L : kernels) {
+        cudaLaunchAttribute attr;
+        const cudaLaunchConfig_t cfg = fill_config(L, 1, nullptr, &attr);
+        FB_CUDA(cudaFuncSetAttribute(fill_kernel(L), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.dynamicSmemBytes));
+        if (clustered(L)) FB_CUDA(cudaFuncSetAttribute(fill_kernel(L), cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    }
+    FB_CUDA(cudaFuncSetAttribute(k_merge_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kFusedWarps * sizeof(WarpShared))));
+    S.cl_cap = probe_cluster({0, DpKernel::Fill, 4, 2}, 8, {16});
+    S.duo_cap = probe_cluster({0, DpKernel::Duo, 8, 2}, 1, {2, 4, 8, 16});
+    S.configured = true;
     return FAMSA_OK;
 }
 
-template <int NW>
-static int launch_cluster_fill(famsa_ctx* ctx, const DpParams& Q, uint32_t cl, cudaStream_t st)
+static int launch_fill(famsa_ctx* ctx, const DpLaunch& L, const DpParams& Q, cudaStream_t st)
 {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(Q.n_jobs * cl);
-    cfg.blockDim = dim3(NW * 32);
-    cfg.dynamicSmemBytes = NW * sizeof(WarpShared);
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = cl;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    FB_CUDA(cudaLaunchKernelEx(&cfg, k_dp_fill<NW, true>, Q));
+    cudaLaunchAttribute attr;
+    const cudaLaunchConfig_t cfg = fill_config(L, Q.n_jobs, st, &attr);
+    cudaLaunchKernelEx(&cfg, fill_kernel(L), Q);
+    FB_CUDA(cudaGetLastError());
     ctx->launches++;
     return FAMSA_OK;
 }
 
-static int launch_duo_fill(famsa_ctx* ctx, const DpParams& Q, uint32_t cl, cudaStream_t st)
+// job k as the kernels see it, offsets left at 0
+static int job_dev(const famsa_dp_job* jobs, const DpJobExt* ext, uint32_t k, DpJobDev& d)
 {
-    static std::atomic<bool> configured[64];
-    if (!configured[ctx->device & 63].load(std::memory_order_acquire)) {
-        FB_CUDA(cudaFuncSetAttribute(k_dp_fill_duo, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDuoSmem));
-        FB_CUDA(cudaFuncSetAttribute(k_dp_fill_duo, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-        configured[ctx->device & 63].store(true, std::memory_order_release);
+    const famsa_dp_job& j = jobs[k];
+    if (j.p1.width == 0 || j.p2.width == 0 || j.p1.card == 0 || j.p2.card == 0) {
+        set_error("dp job " + std::to_string(k) + ": empty profile");
+        return FAMSA_E_INVALID;
     }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(Q.n_jobs * cl);
-    cfg.blockDim = dim3(256);
-    cfg.dynamicSmemBytes = kDuoSmem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = cl;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    FB_CUDA(cudaLaunchKernelEx(&cfg, k_dp_fill_duo, Q));
-    ctx->launches++;
+    d = DpJobDev{reinterpret_cast<const long long*>(j.p1.scores), j.p1.counters, reinterpret_cast<const long long*>(j.p2.scores), j.p2.counters,
+                 j.p1.width, j.p1.card, j.p2.width, j.p2.card,
+                 ext ? ext[k].w1_src : nullptr, ext ? ext[k].w2_src : nullptr, ext ? ext[k].w_dst : nullptr, 0, 0, 0, 0};
     return FAMSA_OK;
 }
 
-// largest cluster size (<= 16) the duo kernel (one block per SM) can be launched with on this device
-static uint32_t max_cluster_duo(famsa_ctx* ctx)
+static DpParams dp_params(const DpJobDev* jobs, DpMeta* meta, uint32_t n, const int64_t gaps[4], unsigned char* sdirs,
+                          unsigned char* path, unsigned char* scratch, famsa_dp_result* results)
 {
-    static std::atomic<int> cached[64];
-    int v = cached[ctx->device & 63].load(std::memory_order_acquire);
-    if (v) return (uint32_t)v;
-    cudaFuncSetAttribute(k_dp_fill_duo, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDuoSmem);
-    cudaFuncSetAttribute(k_dp_fill_duo, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-    v = 1;
-    for (int cl : {2, 4, 8, 16}) {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(cl);
-        cfg.blockDim = dim3(256);
-        cfg.dynamicSmemBytes = kDuoSmem;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = cl; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-        int n = 0;
-        if (cudaOccupancyMaxActiveClusters(&n, k_dp_fill_duo, &cfg) == cudaSuccess && n > 0) v = cl;
-        else { cudaGetLastError(); break; }
-    }
-    cached[ctx->device & 63].store(v, std::memory_order_release);
-    return (uint32_t)v;
-}
-
-// largest cluster size (<= 16) the 4-warp fill kernel can be launched with on this device
-static uint32_t max_cluster4(famsa_ctx* ctx)
-{
-    static std::atomic<int> cached[64];
-    int v = cached[ctx->device & 63].load(std::memory_order_acquire);
-    if (v) return (uint32_t)v;
-    v = 8;
-    for (int cl : {16}) {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(cl);
-        cfg.blockDim = dim3(4 * 32);
-        cfg.dynamicSmemBytes = 4 * sizeof(WarpShared);
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = cl; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-        int n = 0;
-        if (cudaOccupancyMaxActiveClusters(&n, k_dp_fill<4, true>, &cfg) == cudaSuccess && n > 0) v = cl;
-        else cudaGetLastError();
-    }
-    cached[ctx->device & 63].store(v, std::memory_order_release);
-    return (uint32_t)v;
+    DpParams P{};
+    P.jobs = jobs;
+    P.meta = meta;
+    P.n_jobs = n;
+    P.go = gaps[0]; P.ge = gaps[1]; P.to = gaps[2]; P.te = gaps[3];
+    P.sdirs = sdirs;
+    P.path = path;
+    P.scratch = scratch;
+    P.results = results;
+    return P;
 }
 
 unsigned long long dp_scratch_bytes(uint32_t w1, uint32_t w2) { return Scratch(w1, w2).total; }
@@ -1457,24 +1454,19 @@ unsigned long long dp_scratch_bytes(uint32_t w1, uint32_t w2) { return Scratch(w
 // mapped host memory and every device buffer in its own ring (no copy, no allocator call per batch)
 int dp_fused_plan(const famsa_dp_job* jobs, const DpJobExt* ext, uint32_t n, bool align16, DpJobDev* out, DpFusedPlan* plan)
 {
-    unsigned long long path_off = 0, scratch_off = 0, t_off = 0, cells = 0;
+    *plan = DpFusedPlan{};
     for (uint32_t k = 0; k < n; ++k) {
-        const famsa_dp_job& j = jobs[k];
-        if (j.p1.width == 0 || j.p2.width == 0 || j.p1.card == 0 || j.p2.card == 0) { set_error("dp job " + std::to_string(k) + ": empty profile"); return FAMSA_E_INVALID; }
-        DpJobDev& d = out[k];
-        d.s1 = reinterpret_cast<const long long*>(j.p1.scores); d.c1 = j.p1.counters;
-        d.s2 = reinterpret_cast<const long long*>(j.p2.scores); d.c2 = j.p2.counters;
-        d.w1 = j.p1.width; d.card1 = j.p1.card; d.w2 = j.p2.width; d.card2 = j.p2.card;
-        d.w1_src = ext ? ext[k].w1_src : nullptr; d.w2_src = ext ? ext[k].w2_src : nullptr; d.w_dst = ext ? ext[k].w_dst : nullptr;
-        d.path_off = path_off; d.dirs_off = 0;
-        d.scratch_off = scratch_off; d.t_off = t_off;
-        path_off += align16 ? align_up((unsigned long long)d.w1 + d.w2, 16) : (unsigned long long)d.w1 + d.w2;   // 16-byte slots: the traceback
-                                                                       // then stores paths to the host in uint4 units
-        scratch_off += Scratch(d.w1, d.w2).total;
-        t_off += skew_elems(d.w1, d.w2);
-        cells += (unsigned long long)d.w1 * d.w2;
+        DpJobDev d;
+        FB_TRY(job_dev(jobs, ext, k, d));
+        d.path_off = plan->path_bytes;
+        d.scratch_off = plan->scratch_bytes;
+        d.t_off = plan->skew_bytes;
+        plan->path_bytes += path_slot(d.w1, d.w2, align16);
+        plan->scratch_bytes += Scratch(d.w1, d.w2).total;
+        plan->skew_bytes += skew_elems(d.w1, d.w2);
+        plan->cells += (unsigned long long)d.w1 * d.w2;
+        if (out) out[k] = d;
     }
-    plan->scratch_bytes = scratch_off; plan->skew_bytes = t_off; plan->path_bytes = path_off; plan->cells = cells;
     return FAMSA_OK;
 }
 
@@ -1482,21 +1474,9 @@ int dp_fused_launch(famsa_ctx* ctx, const DpJobDev* jobs, uint32_t n, const int6
                     DpMeta* d_meta, uint8_t* d_scratch, uint8_t* d_skew, famsa_dp_result* h_results, uint8_t* h_path,
                     const void* fused_params, uint32_t grid, uint64_t cells, bool record_events, cudaStream_t st)
 {
-    static std::atomic<bool> configured[64];
-    if (!configured[ctx->device & 63].load(std::memory_order_acquire)) {
-        FB_CUDA(cudaFuncSetAttribute(k_merge_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kFusedWarps * sizeof(WarpShared))));
-        configured[ctx->device & 63].store(true, std::memory_order_release);
-    }
+    FB_TRY(dp_setup(ctx));
     ctx->dp.last_cells = cells;
-    DpParams P{};
-    P.jobs = jobs;
-    P.meta = d_meta;
-    P.n_jobs = n;
-    P.go = gaps[0]; P.ge = gaps[1]; P.to = gaps[2]; P.te = gaps[3];
-    P.sdirs = d_skew;
-    P.path = d_path;
-    P.scratch = d_scratch;
-    P.results = d_results;
+    DpParams P = dp_params(jobs, d_meta, n, gaps, d_skew, d_path, d_scratch, d_results);
     P.h_results = h_results;
     P.h_path = h_path;
     if (record_events) { FB_CUDA(cudaEventRecord(ctx->ev[0], st)); FB_CUDA(cudaEventRecord(ctx->ev[1], st)); }
@@ -1507,111 +1487,57 @@ int dp_fused_launch(famsa_ctx* ctx, const DpJobDev* jobs, uint32_t n, const int6
     return FAMSA_OK;
 }
 
-// Bytes of stream-ordered scratch one call of dp_run_device needs at most (it sub-batches above ~1 Gi cells).
+// Bytes of stream-ordered scratch one call of dp_run_device needs at most (it sub-batches above ~4 Gi cells).
 // jobs[k].p1/p2 hold DEVICE pointers here; widths are the layout widths (upper bounds when ext[k].w*_src is set).
 int dp_run_device(famsa_ctx* ctx, const famsa_dp_job* jobs, const DpJobExt* ext, uint32_t n, const int64_t gaps[4],
                   famsa_dp_result* d_results, uint8_t* d_path, uint8_t* d_dirs, DpMeta** d_meta_out, void** d_blob_out,
-                  cudaStream_t st, const void* fused)
+                  cudaStream_t st)
 {
     DpState& S = ctx->dp;
+    const DpKnobs K = dp_knobs();
     std::vector<DpJobDev> dev(n);
+    std::vector<DpGeom> geo(n);
     unsigned long long path_off = 0, dirs_off = 0, cells = 0;
     for (uint32_t k = 0; k < n; ++k) {
-        const famsa_dp_job& j = jobs[k];
-        if (j.p1.width == 0 || j.p2.width == 0 || j.p1.card == 0 || j.p2.card == 0) {
-            set_error("dp job " + std::to_string(k) + ": empty profile");
-            return FAMSA_E_INVALID;
-        }
-        if (((unsigned long long)j.p1.width + 1) * (j.p2.width + 1) > 0xffffffffull) {
+        DpJobDev& d = dev[k];
+        FB_TRY(job_dev(jobs, ext, k, d));
+        if (((unsigned long long)d.w1 + 1) * (d.w2 + 1) > 0xffffffffull) {
             set_error("dp job " + std::to_string(k) + ": more than 2^32 matrix cells");
             return FAMSA_E_INVALID;
         }
-        DpJobDev& d = dev[k];
-        d.s1 = reinterpret_cast<const long long*>(j.p1.scores); d.c1 = j.p1.counters;
-        d.s2 = reinterpret_cast<const long long*>(j.p2.scores); d.c2 = j.p2.counters;
-        d.w1 = j.p1.width; d.card1 = j.p1.card; d.w2 = j.p2.width; d.card2 = j.p2.card;
-        d.w1_src = ext ? ext[k].w1_src : nullptr; d.w2_src = ext ? ext[k].w2_src : nullptr; d.w_dst = ext ? ext[k].w_dst : nullptr;
         d.path_off = path_off; d.dirs_off = dirs_off;           // caller-visible layout: global prefix sums
-        path_off += (unsigned long long)d.w1 + d.w2;
+        path_off += path_slot(d.w1, d.w2, false);
         dirs_off += ((unsigned long long)d.w1 + 1) * (d.w2 + 1);
         cells += (unsigned long long)d.w1 * d.w2;
+        geo[k] = DpGeom{d.w1, d.card1, d.w2, d.card2, Scratch(d.w1, d.w2).total, skew_elems(d.w1, d.w2)};
     }
     S.last_cells = cells;
-    // Sub-batches of consecutive jobs bound the device scratch (direction bytes are 1 byte per cell): ~4 Gi cells each.
-    unsigned long long max_cells = 1ull << 32;
-    if (const char* e = getenv("FAMSA_DP_MAX_CELLS")) max_cells = strtoull(e, nullptr, 10);     // development knob
-    uint32_t team_min = kDpTeamMinWidth;
-    if (const char* e = getenv("FAMSA_DP_TEAM_MIN")) team_min = (uint32_t)atoi(e);               // development knob
-    int nw_forced = 0;
-    if (const char* e = getenv("FAMSA_DP_TEAM_WARPS")) nw_forced = atoi(e);                      // development knob
-    uint32_t cluster_min = kDpClusterMinWidth;
-    if (const char* e = getenv("FAMSA_DP_CLUSTER_MIN")) cluster_min = (uint32_t)atoi(e);         // development knob
-    FB_TRY((configure_fill<1, false>(ctx)));
-    FB_TRY((configure_fill<2, false>(ctx)));
-    FB_TRY((configure_fill<4, false>(ctx)));
-    FB_TRY((configure_fill<kDpTeamWarps, false>(ctx)));
-    FB_TRY((configure_fill<4, true>(ctx)));
-    FB_TRY((configure_fill<kDpTeamWarps, true>(ctx)));
-    {
-        static std::atomic<bool> compact_configured[64];
-        if (!compact_configured[ctx->device & 63].load(std::memory_order_acquire)) {
-            FB_CUDA(cudaFuncSetAttribute(k_dp_fill_compact<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(2 * kCompactStride)));
-            FB_CUDA(cudaFuncSetAttribute(k_dp_fill_compact<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(4 * kCompactStride)));
-            FB_CUDA(cudaFuncSetAttribute(k_dp_fill_compact<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(6 * kCompactStride)));
-            compact_configured[ctx->device & 63].store(true, std::memory_order_release);
-        }
-    }
-    {
-        static std::atomic<bool> configured[64];
-        if (!configured[ctx->device & 63].load(std::memory_order_acquire)) {
-            FB_CUDA(cudaFuncSetAttribute(k_merge_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kFusedWarps * sizeof(WarpShared))));
-            configured[ctx->device & 63].store(true, std::memory_order_release);
-        }
-    }
+    FB_TRY(dp_setup(ctx));
 
-    // plan the sub-batches first: one stream-ordered allocation serves all of them
-    struct Sub { uint32_t j0, j1; unsigned long long scratch, skew; std::vector<unsigned long long> tblock; };
-    std::vector<Sub> subs;
+    // cut the sub-batches first: one stream-ordered allocation serves all of them
+    std::vector<DpSub> subs;
+    if (!dp_cut(K.max_cells, geo, subs)) { set_error("dp sub-batch too large for one launch"); return FAMSA_E_INVALID; }
     unsigned long long max_scratch = 64, max_skew = 64;
     uint32_t max_m = 1;
-    for (uint32_t j0 = 0; j0 < n;) {
-        Sub sb;
-        sb.j0 = j0;
-        uint32_t j1 = j0;
-        unsigned long long mat_sum = 0, scratch_off = 0, t_off = 0;
-        sb.tblock.assign(1, 0);
-        while (j1 < n) {
-            const unsigned long long mat = ((unsigned long long)dev[j1].w1 + 1) * (dev[j1].w2 + 1);
-            if (j1 > j0 && mat_sum + mat > max_cells) break;
-            dev[j1].scratch_off = scratch_off;
-            dev[j1].t_off = t_off;                              // skewed directions are per sub-batch
-            scratch_off += Scratch(dev[j1].w1, dev[j1].w2).total;
-            t_off += skew_elems(dev[j1].w1, dev[j1].w2);
-            mat_sum += mat;
-            sb.tblock.push_back(sb.tblock.back() + (mat + kTThreads * kTCellsPerThread - 1) / (kTThreads * kTCellsPerThread));
-            ++j1;
-        }
-        sb.j1 = j1; sb.scratch = scratch_off; sb.skew = t_off;
-        if (sb.tblock.back() > 0x7fffffffull) { set_error("dp sub-batch too large for one launch"); return FAMSA_E_INVALID; }
-        max_scratch = std::max(max_scratch, scratch_off);
-        max_skew = std::max(max_skew, t_off);
-        max_m = std::max(max_m, j1 - j0);
-        subs.push_back(std::move(sb));
-        j0 = j1;
+    for (const DpSub& sb : subs) {
+        max_scratch = std::max(max_scratch, sb.scratch);
+        max_skew = std::max(max_skew, sb.skew);
+        max_m = std::max(max_m, sb.j1 - sb.j0);
     }
+    for (uint32_t k = 0; k < n; ++k) { dev[k].scratch_off = geo[k].scratch_off; dev[k].t_off = geo[k].t_off; }
     // blob: [jobs n][meta n][order max_m][tblock max_m+1][scratch][skewed dirs]
-    const unsigned long long o_jobs = 0;
-    const unsigned long long o_meta = align_up(o_jobs + sizeof(DpJobDev) * (unsigned long long)std::max(n, 1u), 256);
-    const unsigned long long o_order = align_up(o_meta + sizeof(DpMeta) * (unsigned long long)std::max(n, 1u), 256);
-    const unsigned long long o_tblock = align_up(o_order + sizeof(uint32_t) * (unsigned long long)max_m, 256);
-    const unsigned long long o_scratch = align_up(o_tblock + sizeof(unsigned long long) * ((unsigned long long)max_m + 1), 256);
-    const unsigned long long o_skew = align_up(o_scratch + max_scratch, 256);
-    const unsigned long long blob_bytes = o_skew + max_skew;
+    Layout B;
+    const unsigned long long o_jobs = B.add(sizeof(DpJobDev) * (unsigned long long)std::max(n, 1u));
+    const unsigned long long o_meta = B.add(sizeof(DpMeta) * (unsigned long long)std::max(n, 1u));
+    const unsigned long long o_order = B.add(sizeof(uint32_t) * (unsigned long long)max_m);
+    const unsigned long long o_tblock = B.add(sizeof(unsigned long long) * ((unsigned long long)max_m + 1));
+    const unsigned long long o_scratch = B.add(max_scratch);
+    const unsigned long long o_skew = B.add(max_skew);
     unsigned char* blob = nullptr;
     {
-        cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&blob), blob_bytes, st);
+        cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&blob), B.end, st);
         if (e != cudaSuccess) {
-            set_error("cudaMallocAsync(" + std::to_string(blob_bytes) + ") for the DP scratch failed: " + cudaGetErrorString(e));
+            set_error("cudaMallocAsync(" + std::to_string(B.end) + ") for the DP scratch failed: " + cudaGetErrorString(e));
             return FAMSA_E_NOMEM;
         }
     }
@@ -1620,195 +1546,44 @@ int dp_run_device(famsa_ctx* ctx, const famsa_dp_job* jobs, const DpJobExt* ext,
     FB_CUDA(cudaEventRecord(ctx->ev[0], st));
     FB_CUDA(cudaEventRecord(ctx->ev[1], st));
     if (n) FB_CUDA(cudaMemcpyAsync(d_jobs, dev.data(), sizeof(DpJobDev) * n, cudaMemcpyHostToDevice, st));
-    if (fused) {
-        if (subs.size() != 1 || d_dirs) { set_error("internal: a fused batch must be one sub-batch without CDPMatrix output"); cudaFreeAsync(blob, st); return FAMSA_E_INVALID; }
-        DpParams P{};
-        P.jobs = d_jobs;
-        P.meta = d_meta;
-        P.order = nullptr;
-        P.n_jobs = n;
-        P.job_base = 0;
-        P.go = gaps[0]; P.ge = gaps[1]; P.to = gaps[2]; P.te = gaps[3];
-        P.dirs = nullptr;
-        P.sdirs = blob + o_skew;
-        P.path = d_path;
-        P.scratch = blob + o_scratch;
-        P.tblock = nullptr;
-        P.results = d_results;
-        k_merge_fused<<<n, kFusedWarps * 32, kFusedWarps * sizeof(WarpShared), st>>>(P, *static_cast<const FusedParams*>(fused));
-        FB_CUDA(cudaGetLastError());
-        ctx->launches++;
-        subs.clear();
-    }
-    for (const Sub& sb : subs) {
-        const uint32_t j0 = sb.j0, j1 = sb.j1, m = j1 - j0;
-        // rows of the DP matrix as far as the host can tell (the orientation of ProfProf merges is decided on the device)
-        auto stripes_of = [&](uint32_t a) {
-            const DpJobDev& d = dev[a];
-            const uint32_t rows = d.card1 == 1 ? d.w1 : (d.card2 == 1 ? d.w2 : std::min(d.w1, d.w2));
-            return (rows + 31) / 32;
-        };
-        // Two regimes.  A batch large enough to fill the device with one warp per stripe-pipeline is THROUGHPUT-bound:
-        // wide merges get a block (2, 4 or 8 warps by how many there are), the very widest a cluster of 8 x 8 warps, the
-        // rest run one warp per merge.  A small batch (the chain-like parts and the top of a guide tree, where a level is
-        // one or a few merges) is LATENCY-bound: every merge with more than one stripe gets a cluster of 4-warp blocks,
-        // one stripe per SM sub-partition, as many blocks as its stripes can use (up to 16).
-        uint32_t cl_cap = max_cluster4(ctx);
-        if (const char* e = getenv("FAMSA_DP_MAX_CLUSTER")) cl_cap = std::max(1u, std::min(cl_cap, (uint32_t)atoi(e)));   // development knob
-        // latency mode while the batch's stripes fit one per SM sub-partition
-        unsigned long long demand = 0;
-        uint32_t n_teamable = 0;
-        for (uint32_t a = j0; a < j1; ++a) {
-            demand += std::min(stripes_of(a), 4u * cl_cap);
-            n_teamable += std::min(dev[a].w1, dev[a].w2) > team_min;
-        }
-        bool small_batch = demand <= 4ull * (unsigned long long)ctx->sm_count;
-        if (const char* e = getenv("FAMSA_DP_LATENCY_MODE")) small_batch = atoi(e) != 0;                 // development knob
-        // throughput mode with only a handful of block-sized merges: give every merge with more than 8 stripes a cluster
-        uint32_t cl_min = cluster_min;
-        if (n_teamable * kDpCluster <= 2u * (uint32_t)ctx->sm_count) cl_min = std::min(cluster_min, std::max(team_min, 256u));
-        const bool duo_on = !getenv("FAMSA_DP_DUO") || atoi(getenv("FAMSA_DP_DUO")) != 0;       // development knob (0: one warp per stripe)
-        const uint32_t duo_cap = duo_on ? max_cluster_duo(ctx) : 1;
-        auto cluster_of = [&](uint32_t a) {                       // latency mode: blocks (of 4 warps) for merge a
-            const uint32_t want = (stripes_of(a) + 3) / 4;
-            uint32_t cl = 1;
-            while (cl < want && cl < cl_cap) cl *= 2;
-            return cl;
-        };
-        auto cls = [&](uint32_t a) -> int {                       // sort key: larger = launched first
-            const uint32_t w = std::min(dev[a].w1, dev[a].w2);
-            if (small_batch) {
-                if (stripes_of(a) < 2) return 0;
-                const uint32_t cl = cluster_of(a);
-                // ProfProf merges wide enough for a cluster: producer / consumer pairs (k_dp_fill_duo)
-                if (duo_on && cl >= 2 && dev[a].card1 > 1 && dev[a].card2 > 1) return 100 + (int)std::min(cl, duo_cap);
-                return 10 + (int)cl;
-            }
-            if (w > cl_min) return 2;
-            return w > team_min ? 1 : 0;
-        };
-        std::vector<uint32_t> order(m);
-        std::iota(order.begin(), order.end(), j0);
-        std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) {
-            if (cls(a) != cls(b)) return cls(a) > cls(b);
-            return (unsigned long long)dev[a].w1 * dev[a].w2 > (unsigned long long)dev[b].w1 * dev[b].w2;
-        });
-
-        // Throughput mode: the first wave of blocks lands on the SMs in launch order, so deal the merges (sorted by size) in
-        // snake rows of one block per SM -- the SM that got the largest merge of a row gets the smallest of the next one.
-        if (!small_batch) {
-            const uint32_t sms = (uint32_t)ctx->sm_count;
-            for (uint32_t q0 = 0; q0 < m;) {
-                const int c = cls(order[q0]);
-                uint32_t q1 = q0;
-                while (q1 < m && cls(order[q1]) == c) ++q1;
-                if (c == 1)
-                    for (uint32_t r = q0 + sms, row = 1; r < q1; r += sms, ++row)
-                        if (row & 1) std::reverse(order.begin() + r, order.begin() + std::min(q1, r + sms));
-                q0 = q1;
-            }
-        }
-
+    const DpCaps caps{(uint32_t)ctx->sm_count, S.cl_cap, S.duo_cap, kDpTeamWarps, kDpCluster};
+    for (const DpSub& sb : subs) {
+        const uint32_t m = sb.j1 - sb.j0;
+        const DpSubPlan plan = dp_plan(K, caps, geo, sb);
         // one packed upload: order + tblock
         std::vector<unsigned char> pack(o_scratch - o_order);
-        memcpy(pack.data(), order.data(), sizeof(uint32_t) * m);
+        memcpy(pack.data(), plan.order.data(), sizeof(uint32_t) * m);
         memcpy(pack.data() + (o_tblock - o_order), sb.tblock.data(), sizeof(unsigned long long) * (m + 1));
         FB_CUDA(cudaMemcpyAsync(blob + o_order, pack.data(), (o_tblock - o_order) + sizeof(unsigned long long) * (m + 1), cudaMemcpyHostToDevice, st));
-        DpParams P{};
-        P.jobs = d_jobs;
-        P.meta = d_meta;
+        DpParams P = dp_params(d_jobs, d_meta, m, gaps, blob + o_skew, d_path, blob + o_scratch, d_results);
         P.order = reinterpret_cast<const uint32_t*>(blob + o_order);
-        P.n_jobs = m;
-        P.job_base = j0;
-        P.go = gaps[0]; P.ge = gaps[1]; P.to = gaps[2]; P.te = gaps[3];
+        P.job_base = sb.j0;
         P.dirs = d_dirs;
-        P.sdirs = blob + o_skew;
-        P.path = d_path;
-        P.scratch = blob + o_scratch;
         P.tblock = reinterpret_cast<const unsigned long long*>(blob + o_tblock);
-        P.results = d_results;
         k_dp_prep<<<m, kPrepThreads, 0, st>>>(P);
         FB_CUDA(cudaGetLastError());
         ctx->launches += 1;
-        // one launch per run of equal class in `order`; different classes run side by side (fork after prep, join before
-        // the traceback) so that a level pays for its slowest merge once, not once per launch shape
-        const bool debug = getenv("FAMSA_DP_DEBUG") != nullptr;       // development aid: one line per launch class
-        uint32_t n_classes = 0;
-        for (uint32_t q0 = 0; q0 < m;) { const int c = cls(order[q0]); while (q0 < m && cls(order[q0]) == c) ++q0; ++n_classes; }
-        if (n_classes > 1) FB_CUDA(cudaEventRecord(ctx->ev_fork, st));
-        uint32_t class_no = 0, aux_used = 0;
-        cudaStream_t main_st = st;
-        for (uint32_t q0 = 0; q0 < m;) {
-            const int c = cls(order[q0]);
-            uint32_t q1 = q0;
-            while (q1 < m && cls(order[q1]) == c) ++q1;
-            if (debug) fprintf(stderr, "[dp] batch of %u: class %d x %u (first %u x %u, %u stripes), demand %llu, cl_cap %u, latency_mode %d", m, c, q1 - q0,
-                               dev[order[q0]].w1, dev[order[q0]].w2, stripes_of(order[q0]), demand, cl_cap, (int)small_batch);
-            if (debug && c != 1) fprintf(stderr, "\n");                  // class 1 finishes the line with its team shape below
+        // the launch classes run side by side: fork after prep, join before the traceback
+        if (plan.n_classes > 1) FB_CUDA(cudaEventRecord(ctx->ev_fork, st));
+        uint32_t aux_used = 0;
+        for (const DpLaunch& L : plan.launches) {
+            if (K.debug && !L.wide_only) fputs(dp_debug_line(plan, L, geo).c_str(), stderr);
+            cudaStream_t ls = st;
+            if (L.slot) {
+                const uint32_t a = L.slot - 1;
+                ls = ctx->aux_stream[a];
+                if (!(aux_used >> a & 1)) { FB_CUDA(cudaStreamWaitEvent(ls, ctx->ev_fork, 0)); aux_used |= 1u << a; }
+            }
             DpParams Q = P;
-            Q.order = P.order + q0;
-            Q.n_jobs = q1 - q0;
-            // class 0 (first in launch order is the heaviest) stays on the main stream, the others go to the aux streams
-            cudaStream_t st = main_st;
-            if (class_no > 0) {
-                const uint32_t a = (class_no - 1) % 4;
-                st = ctx->aux_stream[a];
-                if (!(aux_used >> a & 1)) { FB_CUDA(cudaStreamWaitEvent(st, ctx->ev_fork, 0)); aux_used |= 1u << a; }
-            }
-            ++class_no;
-            if (c == 0) {
-                k_dp_fill<1, false><<<(Q.n_jobs + kDpWarps - 1) / kDpWarps, kDpWarps * 32, kDpWarps * sizeof(WarpShared), st>>>(Q);
-                FB_CUDA(cudaGetLastError());
-                ctx->launches++;
-            } else if (c >= 100) {
-                FB_TRY(launch_duo_fill(ctx, Q, (uint32_t)c - 100, st));
-            } else if (c >= 10) {
-                const uint32_t cl = (uint32_t)c - 10;
-                if (cl == 1) {
-                    k_dp_fill<4, false><<<Q.n_jobs, 4 * 32, 4 * sizeof(WarpShared), st>>>(Q);
-                    FB_CUDA(cudaGetLastError());
-                    ctx->launches++;
-                } else FB_TRY(launch_cluster_fill<4>(ctx, Q, cl, st));
-            } else if (c == 2) {
-                FB_TRY(launch_cluster_fill<kDpTeamWarps>(ctx, Q, kDpCluster, st));
-            } else {
-                // Team size by how many merges there are: every SM holds 8 fill warps (shared memory), so a level with many
-                // block-class merges runs them with smaller teams -- 4 warps from 2 merges per SM on, 2 from 4 -- which lose
-                // less to the ramp-up / ramp-down of the stripe pipeline.
-                // From two merges per SM on, the compact kernel (12 warps per SM): 6, 4 or 2 warps per merge.
-                int nw = kDpTeamWarps;
-                const uint32_t sms = (uint32_t)ctx->sm_count;
-                const int compact_mode = getenv("FAMSA_DP_COMPACT") ? atoi(getenv("FAMSA_DP_COMPACT")) : 1;   // development knob: 0 never, 2 always
-                bool compact = compact_mode == 2 || (compact_mode == 1 && Q.n_jobs >= 2u * sms);
-                if (compact) nw = Q.n_jobs >= 6u * sms ? 2 : (Q.n_jobs >= 3u * sms ? 4 : 6);
-                else if (Q.n_jobs >= 4u * sms) nw = 2;
-                else if (Q.n_jobs >= 2u * sms) nw = 4;
-                if (nw_forced) { nw = nw_forced; compact = compact && (nw == 2 || nw == 4 || nw == 6); }
-                if (debug) fprintf(stderr, ", team %d, compact %d\n", nw == 2 || nw == 4 ? nw : (compact ? 6 : kDpTeamWarps), (int)compact);
-                if (compact) {
-                    switch (nw) {
-                    case 2: k_dp_fill_compact<2><<<Q.n_jobs, 2 * 32, 2 * kCompactStride, st>>>(Q); break;
-                    case 4: k_dp_fill_compact<4><<<Q.n_jobs, 4 * 32, 4 * kCompactStride, st>>>(Q); break;
-                    default: k_dp_fill_compact<6><<<Q.n_jobs, 6 * 32, 6 * kCompactStride, st>>>(Q); nw = 4; break;
-                    }
-                    FB_CUDA(cudaGetLastError());
-                    ctx->launches++;
-                    Q.wide_only = 1;                                 // merges whose T needs 8 bytes: the launch below
-                }
-                switch (nw) {
-                case 2: k_dp_fill<2, false><<<Q.n_jobs, 2 * 32, 2 * sizeof(WarpShared), st>>>(Q); break;
-                case 4: k_dp_fill<4, false><<<Q.n_jobs, 4 * 32, 4 * sizeof(WarpShared), st>>>(Q); break;
-                default: k_dp_fill<kDpTeamWarps, false><<<Q.n_jobs, kDpTeamWarps * 32, kDpTeamWarps * sizeof(WarpShared), st>>>(Q); break;
-                }
-                FB_CUDA(cudaGetLastError());
-                ctx->launches++;
-            }
-            q0 = q1;
+            Q.order = P.order + L.q0;
+            Q.n_jobs = L.q1 - L.q0;
+            Q.wide_only = L.wide_only;
+            FB_TRY(launch_fill(ctx, L, Q, ls));
         }
         for (uint32_t a = 0; a < 4; ++a)
             if (aux_used >> a & 1) {
                 FB_CUDA(cudaEventRecord(ctx->ev_join[a], ctx->aux_stream[a]));
-                FB_CUDA(cudaStreamWaitEvent(main_st, ctx->ev_join[a], 0));
+                FB_CUDA(cudaStreamWaitEvent(st, ctx->ev_join[a], 0));
             }
         k_dp_trace<<<(m + kTraceWarps - 1) / kTraceWarps, kTraceWarps * 32, 0, st>>>(P);
         FB_CUDA(cudaGetLastError());

@@ -30,6 +30,7 @@
 #include <deque>
 
 #include "ctx.h"
+#include "dp_plan.h"
 #include "prof_dev.cuh"
 
 namespace fb {
@@ -275,8 +276,7 @@ static cudaEvent_t take_event(ProfState& P)
 // Children of a batch of merges -> DP jobs: resident profiles by their tables (and, while they are still queued, the device
 // slot their width will appear in), leaves by a descriptor for later materialisation.
 static int prof_resolve(famsa_ctx* ctx, const famsa_prof_merge* merges, uint32_t n, std::vector<famsa_dp_job>& jobs, std::vector<DpJobExt>& ext,
-                        std::vector<LeafDesc>& leaves, std::vector<std::pair<uint32_t, int>>& leaf_slot, size_t& leaf_bytes,
-                        uint64_t& path_need, uint64_t& cells)
+                        std::vector<LeafDesc>& leaves, std::vector<std::pair<uint32_t, int>>& leaf_slot, size_t& leaf_bytes)
 {
     ProfState& P = ctx->prof;
     LcsState& L = ctx->lcs;
@@ -308,19 +308,65 @@ static int prof_resolve(famsa_ctx* ctx, const famsa_prof_merge* merges, uint32_t
                 if (e.pending) src = P.d_widths.as<uint32_t>() + c;
             }
         }
-        path_need += (uint64_t)jobs[k].p1.width + jobs[k].p2.width;
-        cells += (uint64_t)jobs[k].p1.width * jobs[k].p2.width;
     }
+    return FAMSA_OK;
+}
+
+// The merged profiles of a batch: one slab, every table sized for the widest alignment possible (w1 + w2 columns),
+// pending until the batch is collected.  Job k publishes its merged width to d_widths[ids[k]]; con[k] (job job_base + k,
+// tile0 left at 0) builds its tables.
+static int place_merged(famsa_ctx* ctx, const std::vector<famsa_dp_job>& jobs, std::vector<DpJobExt>& ext, uint32_t job_base,
+                        std::vector<uint32_t>& ids, std::vector<uint32_t>& gen, std::vector<ConJobDev>& con)
+{
+    ProfState& P = ctx->prof;
+    size_t slab_bytes = 0;
+    for (const famsa_dp_job& j : jobs) slab_bytes += table_bytes(j.p1.width + j.p2.width);
+    int slab;
+    FB_TRY(new_slab(ctx, slab_bytes, &slab));
+    size_t cur = 0;
+    for (uint32_t k = 0; k < (uint32_t)jobs.size(); ++k) {
+        const uint32_t id = new_entry(P);
+        place(P, id, slab, &cur, jobs[k].p1.width + jobs[k].p2.width, jobs[k].p1.card + jobs[k].p2.card);
+        P.entries[id].pending = true;
+        ids.push_back(id);
+        gen.push_back(P.entries[id].gen);
+        ext[k].w_dst = P.d_widths.as<uint32_t>() + id;
+        con.push_back(ConJobDev{P.entries[id].scores, P.entries[id].counters, job_base + k, 0});
+    }
+    return FAMSA_OK;
+}
+
+// The leaf tables of a batch, one after the other from `base`: completes each leaf's descriptor and points its job's
+// side at the tables.
+static void place_leaves(unsigned char* base, std::vector<LeafDesc>& leaves, const std::vector<std::pair<uint32_t, int>>& leaf_slot,
+                         std::vector<famsa_dp_job>& jobs)
+{
+    size_t cur = 0;
+    for (size_t a = 0; a < leaves.size(); ++a) {
+        famsa_dp_profile& p = leaf_slot[a].second ? jobs[leaf_slot[a].first].p2 : jobs[leaf_slot[a].first].p1;
+        char* t = reinterpret_cast<char*>(base + cur);
+        leaves[a].scores = reinterpret_cast<long long*>(t);
+        leaves[a].counters = reinterpret_cast<int*>(t + ((size_t)p.width + 1) * kRows * sizeof(long long));
+        p.scores = reinterpret_cast<const int64_t*>(leaves[a].scores);
+        p.counters = leaves[a].counters;
+        cur += table_bytes(p.width);
+    }
+}
+
+// the children of a batch are consumed (msa.cpp:406-407)
+static int release_children(famsa_ctx* ctx, const famsa_prof_merge* merges, uint32_t n)
+{
+    for (uint32_t k = 0; k < n; ++k)
+        for (uint32_t c : {merges[k].child1, merges[k].child2})
+            if (!(c & FAMSA_PROF_LEAF)) FB_TRY(release_entry(ctx, c));
     return FAMSA_OK;
 }
 
 static bool fused_eligible(const std::vector<famsa_dp_job>& jobs)
 {
     if (jobs.size() > 4096) return false;
-    for (const famsa_dp_job& j : jobs) {
-        const uint32_t rows = j.p1.card == 1 ? j.p1.width : (j.p2.card == 1 ? j.p2.width : std::min(j.p1.width, j.p2.width));
-        if (rows > 512 || std::max(j.p1.width, j.p2.width) > 8192) return false;
-    }
+    for (const famsa_dp_job& j : jobs)
+        if (host_rows(j.p1.width, j.p1.card, j.p2.width, j.p2.card) > 512 || std::max(j.p1.width, j.p2.width) > 8192) return false;
     if (const char* e = getenv("FAMSA_PROF_FUSED")) return atoi(e) != 0;                            // development knob
     return true;
 }
@@ -338,14 +384,13 @@ struct FusedAccum {
     std::vector<uint32_t> merged_ids, merged_gen;
     std::vector<ConJobDev> con;
     size_t leaf_bytes = 0, dev_bytes_est = 0;
-    uint64_t path_bytes = 0;                                         // host path slots used (16-byte aligned when host_mapped)
     uint32_t max_level = 0;
     bool empty() const { return jobs.empty(); }
 };
 
 static size_t fused_dev_estimate(const famsa_dp_job& j)
 {
-    return sizeof(famsa_dp_result) + sizeof(DpMeta) + align_up((uint64_t)j.p1.width + j.p2.width, 16) + 2 * 384ull * (std::max(j.p1.width, j.p2.width) + 2) +
+    return sizeof(famsa_dp_result) + sizeof(DpMeta) + path_slot(j.p1.width, j.p2.width, true) + 2 * 384ull * (std::max(j.p1.width, j.p2.width) + 2) +
            dp_scratch_bytes(j.p1.width, j.p2.width) + skew_elems(j.p1.width, j.p2.width) + 1024;
 }
 
@@ -360,27 +405,12 @@ static bool fused_fits(famsa_ctx* ctx, const FusedAccum& A, const std::vector<fa
 }
 
 static int fused_add(famsa_ctx* ctx, FusedAccum& A, const famsa_prof_merge* merges, uint32_t n, std::vector<famsa_dp_job>& jobs, std::vector<DpJobExt>& ext,
-                     std::vector<LeafDesc>& leaves, std::vector<std::pair<uint32_t, int>>& leaf_slot, size_t leaf_bytes, bool align16)
+                     std::vector<LeafDesc>& leaves, std::vector<std::pair<uint32_t, int>>& leaf_slot, size_t leaf_bytes)
 {
     ProfState& P = ctx->prof;
     const uint32_t base = (uint32_t)A.jobs.size();
-    size_t slab_bytes = 0;
-    for (uint32_t k = 0; k < n; ++k) slab_bytes += table_bytes(jobs[k].p1.width + jobs[k].p2.width);
-    int slab;
-    FB_TRY(new_slab(ctx, slab_bytes, &slab));
-    size_t cur = 0;
-    for (uint32_t k = 0; k < n; ++k) {
-        const uint32_t ub = jobs[k].p1.width + jobs[k].p2.width;
-        const uint32_t id = new_entry(P);
-        place(P, id, slab, &cur, ub, jobs[k].p1.card + jobs[k].p2.card);
-        P.entries[id].pending = true;
-        A.merged_ids.push_back(id);
-        A.merged_gen.push_back(P.entries[id].gen);
-        ext[k].w_dst = P.d_widths.as<uint32_t>() + id;
-        A.con.push_back(ConJobDev{P.entries[id].scores, P.entries[id].counters, base + k, 0});
-        A.dev_bytes_est += fused_dev_estimate(jobs[k]);
-        A.path_bytes += align16 ? align_up((uint64_t)jobs[k].p1.width + jobs[k].p2.width, 16) : (uint64_t)jobs[k].p1.width + jobs[k].p2.width;
-    }
+    FB_TRY(place_merged(ctx, jobs, ext, base, A.merged_ids, A.merged_gen, A.con));
+    for (const famsa_dp_job& j : jobs) A.dev_bytes_est += fused_dev_estimate(j);
     for (auto& ls : leaf_slot) ls.first += base;
     A.jobs.insert(A.jobs.end(), jobs.begin(), jobs.end());
     A.ext.insert(A.ext.end(), ext.begin(), ext.end());
@@ -389,13 +419,10 @@ static int fused_add(famsa_ctx* ctx, FusedAccum& A, const famsa_prof_merge* merg
     A.leaf_bytes += leaf_bytes;
     A.level_start.push_back((uint32_t)A.jobs.size());
     A.max_level = std::max(A.max_level, n);
-    // the children are consumed (msa.cpp:406-407).  Their storage must not be handed out again before this launch has
-    // been queued: inside one launch there is no kernel boundary that would invalidate a stale L1 line
+    // The children's storage must not be handed out again before this launch has been queued: inside one launch there is
+    // no kernel boundary that would invalidate a stale L1 line
     P.arena.defer = true;
-    for (uint32_t k = 0; k < n; ++k)
-        for (uint32_t c : {merges[k].child1, merges[k].child2})
-            if (!(c & FAMSA_PROF_LEAF)) FB_TRY(release_entry(ctx, c));
-    return FAMSA_OK;
+    return release_children(ctx, merges, n);
 }
 
 static int fused_flush(famsa_ctx* ctx, FusedAccum& A, const int64_t gaps[4], famsa_dp_result* h_results, uint8_t* h_paths, bool host_mapped, ProfTicket* T)
@@ -404,43 +431,30 @@ static int fused_flush(famsa_ctx* ctx, FusedAccum& A, const int64_t gaps[4], fam
     LcsState& L = ctx->lcs;
     cudaStream_t st = ctx->stream;
     const uint32_t n = (uint32_t)A.jobs.size(), n_levels = (uint32_t)A.level_start.size() - 1;
-    std::vector<DpJobDev> plan_jobs(n);
     DpFusedPlan plan;
-    FB_TRY(dp_fused_plan(A.jobs.data(), A.ext.data(), n, host_mapped, plan_jobs.data(), &plan));
-    const size_t ho_fj = align_up(sizeof(DpJobDev) * n, 256);
-    const size_t ho_lv = align_up(ho_fj + sizeof(FusedJob) * n, 256);
-    const size_t h_bytes = ho_lv + sizeof(uint32_t) * (n_levels + 1);
-    const size_t o_res = 0;
-    const size_t o_meta = align_up(o_res + sizeof(famsa_dp_result) * n, 256);
-    const size_t o_path = align_up(o_meta + sizeof(DpMeta) * n, 256);
-    const size_t o_leaf = align_up(o_path + std::max<uint64_t>(plan.path_bytes, 1), 256);
-    const size_t o_scr = align_up(o_leaf + A.leaf_bytes, 256);
-    const size_t o_skew = align_up(o_scr + plan.scratch_bytes, 256);
-    const size_t d_bytes = o_skew + plan.skew_bytes;
-    const size_t h_off = P.h_ring.alloc(h_bytes), d_off = P.d_ring.alloc(d_bytes);
+    FB_TRY(dp_fused_plan(A.jobs.data(), A.ext.data(), n, host_mapped, nullptr, &plan));
+    Layout H, D;
+    const size_t ho_jobs = H.add(sizeof(DpJobDev) * n);
+    const size_t ho_fj = H.add(sizeof(FusedJob) * n);
+    const size_t ho_lv = H.add(sizeof(uint32_t) * (n_levels + 1));
+    const size_t o_res = D.add(sizeof(famsa_dp_result) * n);
+    const size_t o_meta = D.add(sizeof(DpMeta) * n);
+    const size_t o_path = D.add(std::max<uint64_t>(plan.path_bytes, 1));
+    const size_t o_leaf = D.add(A.leaf_bytes);
+    const size_t o_scr = D.add(plan.scratch_bytes);
+    const size_t o_skew = D.add(plan.skew_bytes);
+    const size_t h_off = P.h_ring.alloc(H.end), d_off = P.d_ring.alloc(D.end);
     if (h_off == (size_t)-1 || d_off == (size_t)-1) { set_error("internal: the fused batch does not fit its rings"); return FAMSA_E_NOMEM; }
     unsigned char* hb = P.h_ring_mem + h_off;
     unsigned char* db = P.d_ring_mem.as<unsigned char>() + d_off;
-    DpJobDev* hj = reinterpret_cast<DpJobDev*>(hb);
+    DpJobDev* hj = reinterpret_cast<DpJobDev*>(hb + ho_jobs);
     FusedJob* fj = reinterpret_cast<FusedJob*>(hb + ho_fj);
     uint32_t* hl = reinterpret_cast<uint32_t*>(hb + ho_lv);
     famsa_dp_result* d_results = reinterpret_cast<famsa_dp_result*>(db + o_res);
+    place_leaves(db + o_leaf, A.leaves, A.leaf_slot, A.jobs);
+    FB_TRY(dp_fused_plan(A.jobs.data(), A.ext.data(), n, host_mapped, hj, &plan));    // now with the leaves' tables
     for (uint32_t k = 0; k < n; ++k) { fj[k].leaf[0].seq = fj[k].leaf[1].seq = 0xffffffffu; fj[k].con = A.con[k]; }
-    size_t cur = 0;
-    for (size_t a = 0; a < A.leaves.size(); ++a) {
-        const uint32_t k = A.leaf_slot[a].first;
-        const int side = A.leaf_slot[a].second;
-        const uint32_t w = side ? A.jobs[k].p2.width : A.jobs[k].p1.width;
-        char* base = reinterpret_cast<char*>(db + o_leaf + cur);
-        LeafDesc ld = A.leaves[a];
-        ld.scores = reinterpret_cast<long long*>(base);
-        ld.counters = reinterpret_cast<int*>(base + ((size_t)w + 1) * kRows * sizeof(long long));
-        (side ? plan_jobs[k].s2 : plan_jobs[k].s1) = ld.scores;
-        (side ? plan_jobs[k].c2 : plan_jobs[k].c1) = ld.counters;
-        fj[k].leaf[side] = ld;
-        cur += table_bytes(w);
-    }
-    memcpy(hj, plan_jobs.data(), sizeof(DpJobDev) * n);
+    for (size_t a = 0; a < A.leaves.size(); ++a) fj[A.leaf_slot[a].first].leaf[A.leaf_slot[a].second] = A.leaves[a];
     memcpy(hl, A.level_start.data(), sizeof(uint32_t) * (n_levels + 1));
     FusedParams FP{fj, hl, n_levels, L.d_raw_codes.as<int8_t>(), L.d_raw_off.as<uint64_t>(), L.d_raw_len.as<uint32_t>(), P.d_sm.as<long long>(),
                    0, P.d_block_counter.as<unsigned>(), nullptr, 0};
@@ -498,11 +512,11 @@ static int prof_launch(famsa_ctx* ctx, const famsa_prof_merge* merges, uint32_t 
     std::vector<LeafDesc> leaves;
     std::vector<std::pair<uint32_t, int>> leaf_slot;                 // (job, side) per leaf, in `leaves` order
     size_t leaf_bytes = 0;
+    FB_TRY(prof_resolve(ctx, merges, n, jobs, ext, leaves, leaf_slot, leaf_bytes));
     uint64_t path_need = 0, cells = 0;
-    FB_TRY(prof_resolve(ctx, merges, n, jobs, ext, leaves, leaf_slot, leaf_bytes, path_need, cells));
-    if (host_mapped) {
-        path_need = 0;
-        for (uint32_t k = 0; k < n; ++k) path_need += align_up((uint64_t)jobs[k].p1.width + jobs[k].p2.width, 16);
+    for (const famsa_dp_job& j : jobs) {
+        path_need += path_slot(j.p1.width, j.p2.width, host_mapped);
+        cells += (uint64_t)j.p1.width * j.p2.width;
     }
     if (path_need > path_cap) {
         set_error("famsa_prof_merge_batch: path_buf holds " + std::to_string(path_cap) + " bytes, " + std::to_string(path_need) + " needed");
@@ -511,77 +525,43 @@ static int prof_launch(famsa_ctx* ctx, const famsa_prof_merge* merges, uint32_t 
     FB_TRY(ensure_widths(ctx, P.entries.size() + n));
     // A batch of small merges only (the chain-like parts of a guide tree: every level one or a few short merges) runs
     // every merge whole in one block of k_merge_fused instead of five launches.
-    bool fused = fused_eligible(jobs);
-    if (fused) {
+    if (fused_eligible(jobs)) {
         FB_TRY(ensure_rings(ctx));
         FusedAccum A;
         if (fused_fits(ctx, A, jobs)) {
-            FB_TRY(fused_add(ctx, A, merges, n, jobs, ext, leaves, leaf_slot, leaf_bytes, host_mapped));
+            FB_TRY(fused_add(ctx, A, merges, n, jobs, ext, leaves, leaf_slot, leaf_bytes));
             return fused_flush(ctx, A, gaps, h_results, h_paths, host_mapped, T);
         }
     }
-    // merged tables: one slab per batch, every profile sized for the widest alignment possible (w1 + w2 columns)
-    size_t slab_bytes = 0;
-    for (uint32_t k = 0; k < n; ++k) slab_bytes += table_bytes(jobs[k].p1.width + jobs[k].p2.width);
-    int slab;
-    FB_TRY(new_slab(ctx, slab_bytes, &slab));
-    fused = false;                                                   // (the launch-by-launch path below)
+    std::vector<ConJobDev> con;
+    FB_TRY(place_merged(ctx, jobs, ext, 0, T->merged_ids, T->merged_gen, con));
+    uint32_t tiles = 0;
+    for (uint32_t k = 0; k < n; ++k) {
+        con[k].tile0 = tiles;
+        tiles += (jobs[k].p1.width + jobs[k].p2.width + 1 + kConTile - 1) / kConTile;
+    }
     // batch blob: [results][con jobs][leaf descs][paths][leaf tables]
-    const size_t o_res = 0;
-    const size_t o_con = align_up(o_res + sizeof(famsa_dp_result) * n, 256);
-    const size_t o_leafd = align_up(o_con + (fused ? sizeof(FusedJob) : sizeof(ConJobDev)) * n, 256);
-    const size_t o_path = align_up(o_leafd + sizeof(LeafDesc) * leaves.size(), 256);
-    const size_t o_leaf = align_up(o_path + std::max<uint64_t>(path_need, 1), 256);
-    const size_t blob_bytes = o_leaf + leaf_bytes;
+    Layout B;
+    const size_t o_res = B.add(sizeof(famsa_dp_result) * n);
+    const size_t o_con = B.add(sizeof(ConJobDev) * n);
+    const size_t o_leafd = B.add(sizeof(LeafDesc) * leaves.size());
+    const size_t o_path = B.add(std::max<uint64_t>(path_need, 1));
+    const size_t o_leaf = B.add(leaf_bytes);
     unsigned char* blob = nullptr;
     {
-        cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&blob), blob_bytes, st);
+        cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&blob), B.end, st);
         if (e != cudaSuccess) { set_error(std::string("cudaMallocAsync for a merge batch failed: ") + cudaGetErrorString(e)); return FAMSA_E_NOMEM; }
     }
     famsa_dp_result* d_results = reinterpret_cast<famsa_dp_result*>(blob + o_res);
     uint8_t* d_path = blob + o_path;
-
+    place_leaves(blob + o_leaf, leaves, leaf_slot, jobs);
+    // one upload: construct jobs and leaf descriptors
     std::vector<unsigned char> pack(o_path - o_con);
-    std::vector<ConJobDev> cj_store(n);
-    ConJobDev* cj = cj_store.data();
-    FusedJob* fj = reinterpret_cast<FusedJob*>(pack.data());
-    LeafDesc* ld = reinterpret_cast<LeafDesc*>(pack.data() + (o_leafd - o_con));
-    if (fused)
-        for (uint32_t k = 0; k < n; ++k) fj[k].leaf[0].seq = fj[k].leaf[1].seq = 0xffffffffu;
-    {
-        size_t cur = 0;
-        for (size_t a = 0; a < leaves.size(); ++a) {
-            famsa_dp_profile& p = leaf_slot[a].second ? jobs[leaf_slot[a].first].p2 : jobs[leaf_slot[a].first].p1;
-            char* base = reinterpret_cast<char*>(blob + o_leaf + cur);
-            leaves[a].scores = reinterpret_cast<long long*>(base);
-            leaves[a].counters = reinterpret_cast<int*>(base + ((size_t)p.width + 1) * kRows * sizeof(long long));
-            p.scores = reinterpret_cast<const int64_t*>(leaves[a].scores);
-            p.counters = leaves[a].counters;
-            cur += table_bytes(p.width);
-            ld[a] = leaves[a];
-            if (fused) fj[leaf_slot[a].first].leaf[leaf_slot[a].second] = leaves[a];
-        }
-    }
-    T->merged_ids.assign(n, 0);
-    T->merged_gen.assign(n, 0);
-    size_t cur = 0;
-    uint32_t tiles = 0;
-    for (uint32_t k = 0; k < n; ++k) {
-        const uint32_t ub = jobs[k].p1.width + jobs[k].p2.width;
-        const uint32_t id = new_entry(P);
-        place(P, id, slab, &cur, ub, jobs[k].p1.card + jobs[k].p2.card);
-        P.entries[id].pending = true;
-        T->merged_ids[k] = id;
-        T->merged_gen[k] = P.entries[id].gen;
-        ext[k].w_dst = P.d_widths.as<uint32_t>() + id;
-        cj[k].os = P.entries[id].scores; cj[k].oc = P.entries[id].counters; cj[k].job = k; cj[k].tile0 = tiles;
-        tiles += (ub + 1 + kConTile - 1) / kConTile;
-        if (fused) fj[k].con = cj[k];
-    }
-    if (!fused) memcpy(pack.data(), cj, sizeof(ConJobDev) * n);
+    memcpy(pack.data(), con.data(), sizeof(ConJobDev) * n);
+    memcpy(pack.data() + (o_leafd - o_con), leaves.data(), sizeof(LeafDesc) * leaves.size());
     FB_CUDA(cudaEventRecord(P.ev[0], st));
     FB_CUDA(cudaMemcpyAsync(blob + o_con, pack.data(), pack.size(), cudaMemcpyHostToDevice, st));
-    if (!leaves.empty() && !fused) {
+    if (!leaves.empty()) {
         k_prof_leaf<<<(unsigned)leaves.size(), 256, 0, st>>>(reinterpret_cast<const LeafDesc*>(blob + o_leafd), L.d_raw_codes.as<int8_t>(),
                                                              L.d_raw_off.as<uint64_t>(), L.d_raw_len.as<uint32_t>(),
                                                              P.d_sm.as<long long>(), gaps[0], gaps[1], gaps[2], gaps[3]);
@@ -593,22 +573,17 @@ static int prof_launch(famsa_ctx* ctx, const famsa_prof_merge* merges, uint32_t 
     void* dp_blob = nullptr;
     FB_TRY(dp_run_device(ctx, jobs.data(), ext.data(), n, gaps, d_results, d_path, nullptr, &d_meta, &dp_blob, st));
     FB_CUDA(cudaEventRecord(P.ev[1], st));
-    if (!fused) {
-        k_prof_construct<<<tiles, kConThreads, 0, st>>>(reinterpret_cast<const ConJobDev*>(blob + o_con), n, d_meta, d_results, d_path,
-                                                        gaps[0], gaps[1], gaps[2], gaps[3]);
-        FB_CUDA(cudaGetLastError());
-        ++ctx->launches;
-    }
+    k_prof_construct<<<tiles, kConThreads, 0, st>>>(reinterpret_cast<const ConJobDev*>(blob + o_con), n, d_meta, d_results, d_path,
+                                                    gaps[0], gaps[1], gaps[2], gaps[3]);
+    FB_CUDA(cudaGetLastError());
+    ++ctx->launches;
     FB_CUDA(cudaEventRecord(P.ev[2], st));
     P.timing_valid = true;
     FB_CUDA(cudaMemcpyAsync(h_results, d_results, sizeof(famsa_dp_result) * n, cudaMemcpyDeviceToHost, st));
     if (path_need) FB_CUDA(cudaMemcpyAsync(h_paths, d_path, path_need, cudaMemcpyDeviceToHost, st));
     FB_CUDA(cudaFreeAsync(dp_blob, st));
     FB_CUDA(cudaFreeAsync(blob, st));
-    // the children are consumed (msa.cpp:406-407); frees are ordered after the construct kernel
-    for (uint32_t k = 0; k < n; ++k)
-        for (uint32_t c : {merges[k].child1, merges[k].child2})
-            if (!(c & FAMSA_PROF_LEAF)) FB_TRY(release_entry(ctx, c));
+    FB_TRY(release_children(ctx, merges, n));                        // frees are ordered after the construct kernel
     T->done = take_event(P);
     FB_CUDA(cudaEventRecord(T->done, st));
     T->n = n; T->h_results = h_results; T->h_paths = h_paths; T->path_bytes = path_need; T->cells_bound = cells;
@@ -736,6 +711,7 @@ int prof_align_tree(famsa_ctx* ctx, const int32_t* tree, uint32_t n_leaves, cons
     double t_collect = 0, t_launch = 0;
     uint32_t max_exact = 0;                                         // widest profile whose real width is known
     for (uint32_t i = 0; i < n_leaves; ++i) max_exact = std::max(max_exact, width[i]);
+    const bool debug = getenv("FAMSA_DP_DEBUG") != nullptr;       // development aid: [tree] lines on stderr
     auto now = []() { return std::chrono::steady_clock::now(); };
     auto collect_front = [&]() -> int {
         InFlight& f = q.front();
@@ -754,6 +730,7 @@ int prof_align_tree(famsa_ctx* ctx, const int32_t* tree, uint32_t n_leaves, cons
         q.pop_front();
         return rc;
     };
+    auto finished = [&](const ProfTicket& t) { return t.done_seq ? *P.h_done >= t.done_seq : (!t.done || cudaEventQuery(t.done) == cudaSuccess); };
     int rc = FAMSA_OK;
     // paths of all merges: one pinned arena, grown only while nothing is in flight
     uint64_t arena_need = 0;
@@ -779,7 +756,7 @@ int prof_align_tree(famsa_ctx* ctx, const int32_t* tree, uint32_t n_leaves, cons
         f.merge_ids = acc_merges;
         f.path_base = acc_path_base;
         f.res_base = acc_res_base;
-        if (getenv("FAMSA_DP_DEBUG")) fprintf(stderr, "[tree] fused launch: %u levels, %zu merges\n", acc_levels, acc.jobs.size());
+        if (debug) fprintf(stderr, "[tree] fused launch: %u levels, %zu merges\n", acc_levels, acc.jobs.size());
         const auto t0 = now();
         const int r = fused_flush(ctx, acc, gaps, P.h_tree_results + acc_res_base, P.h_tree_paths + acc_path_base, true, &f.t);
         t_launch += std::chrono::duration<double, std::micro>(now() - t0).count();
@@ -792,9 +769,13 @@ int prof_align_tree(famsa_ctx* ctx, const int32_t* tree, uint32_t n_leaves, cons
     };
     for (size_t lv = 0; lv < levels.size() && rc == FAMSA_OK; ++lv) {
         const std::vector<uint32_t>& level = levels[lv];
+        std::vector<famsa_prof_merge> mg(level.size());             // the level's merges by their children's handles
+        for (size_t a = 0; a < level.size(); ++a) {
+            mg[a].child1 = handle[(uint32_t)tree[2 * level[a]]];
+            mg[a].child2 = handle[(uint32_t)tree[2 * level[a] + 1]];
+        }
         {
             // small merges: join the accumulation when the level fits
-            auto finished = [&](const ProfTicket& t) { return t.done_seq ? *P.h_done >= t.done_seq : (!t.done || cudaEventQuery(t.done) == cudaSuccess); };
             while (!q.empty() && finished(q.front().t) && rc == FAMSA_OK) rc = collect_front();
             if (rc) break;
             // A queued child is known by an upper bound only (the sum of its children's bounds), and along a chain the bounds
@@ -812,22 +793,15 @@ int prof_align_tree(famsa_ctx* ctx, const int32_t* tree, uint32_t n_leaves, cons
                 if (rc) break;
                 ++n_drains;
             }
-            std::vector<famsa_prof_merge> mg(level.size());
-            for (size_t a = 0; a < level.size(); ++a) {
-                const uint32_t k = level[a];
-                mg[a].child1 = handle[(uint32_t)tree[2 * k]];
-                mg[a].child2 = handle[(uint32_t)tree[2 * k + 1]];
-            }
             std::vector<famsa_dp_job> jobs;
             std::vector<DpJobExt> ext;
             std::vector<LeafDesc> leaves;
             std::vector<std::pair<uint32_t, int>> leaf_slot;
             size_t leaf_bytes = 0;
-            uint64_t pn = 0, cl = 0;
-            rc = prof_resolve(ctx, mg.data(), (uint32_t)mg.size(), jobs, ext, leaves, leaf_slot, leaf_bytes, pn, cl);
+            rc = prof_resolve(ctx, mg.data(), (uint32_t)mg.size(), jobs, ext, leaves, leaf_slot, leaf_bytes);
             if (rc) break;
             uint64_t path_need = 0;
-            for (const famsa_dp_job& j : jobs) path_need += align_up((uint64_t)j.p1.width + j.p2.width, 16);
+            for (const famsa_dp_job& j : jobs) path_need += path_slot(j.p1.width, j.p2.width, true);
             if (fused_eligible(jobs) && path_cursor + path_need <= P.h_tree_paths_cap) {
                 if (!(acc_levels < kMaxFusedLevels && acc.jobs.size() + jobs.size() <= 8192 && fused_fits(ctx, acc, jobs))) {
                     rc = flush_acc();
@@ -839,7 +813,7 @@ int prof_align_tree(famsa_ctx* ctx, const int32_t* tree, uint32_t n_leaves, cons
                 if (fused_fits(ctx, acc, jobs)) {
                     if (acc.empty()) { acc_path_base = path_cursor; acc_res_base = res_cursor; }
                     const size_t first = acc.merged_ids.size();
-                    rc = fused_add(ctx, acc, mg.data(), (uint32_t)mg.size(), jobs, ext, leaves, leaf_slot, leaf_bytes, true);
+                    rc = fused_add(ctx, acc, mg.data(), (uint32_t)mg.size(), jobs, ext, leaves, leaf_slot, leaf_bytes);
                     if (rc) break;
                     for (size_t a = 0; a < level.size(); ++a) {
                         const uint32_t k = level[a];
@@ -854,12 +828,11 @@ int prof_align_tree(famsa_ctx* ctx, const int32_t* tree, uint32_t n_leaves, cons
                     continue;
                 }
             }
-            if (getenv("FAMSA_DP_DEBUG")) fprintf(stderr, "[tree] level %zu (%zu merges) not fused: eligible %d, path room %d\n", lv, level.size(), (int)fused_eligible(jobs), (int)(path_cursor + path_need <= P.h_tree_paths_cap)), fprintf(stderr, "        first job: %u (card %u) x %u (card %u)\n", jobs[0].p1.width, jobs[0].p1.card, jobs[0].p2.width, jobs[0].p2.card);
+            if (debug) fprintf(stderr, "[tree] level %zu (%zu merges) not fused: eligible %d, path room %d\n", lv, level.size(), (int)fused_eligible(jobs), (int)(path_cursor + path_need <= P.h_tree_paths_cap)), fprintf(stderr, "        first job: %u (card %u) x %u (card %u)\n", jobs[0].p1.width, jobs[0].p1.card, jobs[0].p2.width, jobs[0].p2.card);
             rc = flush_acc();                                         // this level goes launch by launch: everything before it first
             if (rc) break;
         }
         // collect whatever has finished already (tightens the bounds for free)
-        auto finished = [&](const ProfTicket& t) { return t.done_seq ? *P.h_done >= t.done_seq : (!t.done || cudaEventQuery(t.done) == cudaSuccess); };
         while (!q.empty() && finished(q.front().t) && rc == FAMSA_OK) rc = collect_front();
         if (rc) break;
         auto level_cost = [&](uint64_t* bound_cells, uint64_t* path_need) {
@@ -867,7 +840,7 @@ int prof_align_tree(famsa_ctx* ctx, const int32_t* tree, uint32_t n_leaves, cons
             for (uint32_t k : level) {
                 const uint32_t a = (uint32_t)tree[2 * k], b = (uint32_t)tree[2 * k + 1];
                 *bound_cells += (uint64_t)width[a] * width[b];
-                *path_need += align_up((uint64_t)width[a] + width[b], 16);
+                *path_need += path_slot(width[a], width[b], true);
             }
         };
         uint64_t bound_cells, path_need;
@@ -895,12 +868,6 @@ int prof_align_tree(famsa_ctx* ctx, const int32_t* tree, uint32_t n_leaves, cons
                 cudaFreeHost(old);
             }
         }
-        std::vector<famsa_prof_merge> mg(level.size());
-        for (size_t a = 0; a < level.size(); ++a) {
-            const uint32_t k = level[a];
-            mg[a].child1 = handle[(uint32_t)tree[2 * k]];
-            mg[a].child2 = handle[(uint32_t)tree[2 * k + 1]];
-        }
         q.emplace_back();
         InFlight& f = q.back();
         f.merge_ids = level;
@@ -925,7 +892,7 @@ int prof_align_tree(famsa_ctx* ctx, const int32_t* tree, uint32_t n_leaves, cons
     if (rc == FAMSA_OK) rc = flush_acc();
     while (!q.empty()) { const int r2 = collect_front(); if (rc == FAMSA_OK) rc = r2; }
     if (rc) return rc;
-    if (getenv("FAMSA_DP_DEBUG"))
+    if (debug)
         fprintf(stderr, "[tree] host time: %.0f us in prof_launch, %.0f us waiting in prof_collect, %.0f us total so far, %u batches\n", t_launch, t_collect,
                 std::chrono::duration<double, std::micro>(now() - t_begin).count(), n_batches);
     FB_CUDA(cudaEventRecord(P.ev_tree[1], ctx->stream));
