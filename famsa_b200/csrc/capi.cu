@@ -519,7 +519,7 @@ int famsa_lcs_upgma(famsa_ctx* ctx, int distance_kind, int modified, int32_t* tr
     return entry(ctx, nullptr, &famsa_ctx::lcs_timing, [&]() -> int {
         FB_TRY(check_set(ctx, 2));
         if (!tree) { set_error("NULL argument"); return FAMSA_E_INVALID; }
-        if (distance_kind < 0 || distance_kind > 2) { set_error("distance_kind must be 0, 1 or 2"); return FAMSA_E_INVALID; }
+        if (distance_kind != 0 && distance_kind != 1) { set_error("UPGMA is instantiated for distance_kind 0 and 1 only"); return FAMSA_E_INVALID; }
         return FAMSA_OK;
     }, [&](cudaStream_t st) -> int {
         ctx->lcs.last_pairs = tri(ctx->lcs.n);
@@ -532,7 +532,7 @@ int famsa_lcs_upgma_from_triangle(famsa_ctx* ctx, int distance_kind, int modifie
     return entry(ctx, nullptr, &famsa_ctx::lcs_timing, [&]() -> int {
         FB_TRY(check_set(ctx, 2));
         if (!tree || !d_triangle) { set_error("NULL argument"); return FAMSA_E_INVALID; }
-        if (distance_kind < 0 || distance_kind > 2) { set_error("distance_kind must be 0, 1 or 2"); return FAMSA_E_INVALID; }
+        if (distance_kind != 0 && distance_kind != 1) { set_error("UPGMA is instantiated for distance_kind 0 and 1 only"); return FAMSA_E_INVALID; }
         return check_elem(elem_bytes, 2);                               // the caller's triangle: any width the caller chose
     }, [&](cudaStream_t st) -> int {
         ctx->lcs.last_pairs = 0;

@@ -177,10 +177,14 @@ int famsa_lcs_prim(famsa_ctx* ctx, int distance_kind, int32_t* edge_from, int32_
  * leaves the device, only the n-1 merges return.  tree[2k], tree[2k+1] = children of internal node n_seqs + k (node ids as
  * in tree_structure: leaves 0..n-1 in caller order, which must be the order the reference builds the tree on -- length
  * descending, src/msa.cpp:245-256); the result is the reference's tree pair for pair, including the stale-cache behaviour
- * of its scans.  distance_kind as in famsa_transform_f32 (0 or 1 are what UPGMA is instantiated for).  HOST pointer. */
+ * of its scans.  distance_kind 0 (indel075_div_lcs) or 1 (indel_div_lcs), the two UPGMA instantiations; 2 (pairwise
+ * identity, a similarity) is rejected with FAMSA_E_INVALID.  When no live row has a finite cached distance left (e.g. a
+ * sequence without a common residue with any other; there the reference would index out of range) the call returns
+ * FAMSA_E_INVALID and the context stays usable.  HOST pointer. */
 int famsa_lcs_upgma(famsa_ctx* ctx, int distance_kind, int modified, int32_t* tree);
 /* Same on a packed LCS triangle that is already in HBM (DEVICE pointer; layout and elem_bytes as famsa_lcs_triangle_device
- * writes it for rows 0..n_seqs) -- e.g. the triangle a multi-GPU run has just all-gathered. */
+ * writes it for rows 0..n_seqs) -- e.g. the triangle a multi-GPU run has just all-gathered.  The values are not checked:
+ * they must be LCS lengths of the uploaded set (distance kind 0 looks up pow(indel, 0.75) in a table sized by its lengths). */
 int famsa_lcs_upgma_from_triangle(famsa_ctx* ctx, int distance_kind, int modified, const void* d_triangle, int elem_bytes,
                                   int32_t* tree);
 

@@ -19,6 +19,7 @@
  *                         minus the Transform)
  *   lcs_oracle_triangle   src/tree/AbstractTreeGenerator.hpp:379-398 (calculateDistanceMatrix)
  *   lcs_oracle_transform_*  src/tree/AbstractTreeGenerator.hpp:28-82 (Transform<T, Distance>)
+ *   lcs_oracle_transform_tri_f32  the same Transform<float> over a packed triangle (UPGMA.cpp:75-109, computeDistances)
  *
  * Residue codes: 0..23 ("ARNDCQEGHILKMFPSTWYVBZX*", sequence.cpp:17), 22 = unknown / padding.
  * Only codes < 20 ever set a mask bit (sequence.cpp:199).
@@ -142,4 +143,40 @@ float lcs_oracle_transform_f32(int kind, uint32_t lcs, uint32_t len1, uint32_t l
     /* table entry is (float) pow((double) i, 0.75), hpp:46 */
     if (kind == 0) return (float)pow((double)(uint32_t)indel, 0.75) / (float)lcs;
     return indel / lcs;
+}
+
+/* lcs_oracle_transform_f32 of every pair of a packed LCS triangle (rows 0..n, elem_bytes 2 or 4, row i at i(i-1)/2):
+ * out[i(i-1)/2 + j] = Transform(lcs, lens[i], lens[j]) -- the float triangle computeDistances fills
+ * (src/tree/UPGMA.cpp:75-109) -- with the pow table built once instead of per pair. */
+void lcs_oracle_transform_tri_f32(int kind, const void *lcs, int elem_bytes, const uint32_t *lens, uint32_t n,
+                                  float *out)
+{
+    uint32_t max_len = 0;
+    for (uint32_t i = 0; i < n; ++i) max_len = lens[i] > max_len ? lens[i] : max_len;
+    float *pow075 = NULL;
+    if (kind == 0) {
+        pow075 = (float *)malloc(sizeof(float) * (2 * (size_t)max_len + 1));
+        for (size_t k = 0; k <= 2 * (size_t)max_len; ++k) pow075[k] = (float)pow((double)k, 0.75);
+    }
+    const float never = (float)nextafter((double)FLT_MAX, 0.0);
+    for (uint32_t i = 1; i < n; ++i) {
+        const size_t base = (size_t)i * (i - 1) / 2;
+        for (uint32_t j = 0; j < i; ++j) {
+            const uint32_t l = elem_bytes == 2 ? ((const uint16_t *)lcs)[base + j] : ((const uint32_t *)lcs)[base + j];
+            float d;
+            if (kind == 2) {
+                const uint32_t m = lens[i] < lens[j] ? lens[i] : lens[j];
+                d = (float)l / m;
+            } else if (!l) {
+                d = never;
+            } else {
+                const uint32_t indel = lens[i] + lens[j] - 2 * l;       /* wraps as in the scalar form */
+                const float p = kind != 0 ? 0.0f
+                              : indel <= 2 * max_len ? pow075[indel] : (float)pow((double)(uint32_t)(float)indel, 0.75);
+                d = kind == 0 ? p / (float)l : (float)indel / l;
+            }
+            out[base + j] = d;
+        }
+    }
+    free(pow075);
 }

@@ -43,6 +43,9 @@ def oracle() -> C.CDLL:
         lib.lcs_oracle_transform_f64.restype = C.c_double
         lib.lcs_oracle_transform_f32.argtypes = [C.c_int, u32, u32, u32]
         lib.lcs_oracle_transform_f32.restype = C.c_float
+        lib.lcs_oracle_transform_tri_f32.argtypes = [C.c_int, vp, C.c_int, vp, u32, vp]
+        lib.upgma_oracle_tree.argtypes = [vp, u32, C.c_int, C.c_int, C.c_int, vp, vp]
+        lib.upgma_oracle_tree.restype = C.c_int
         lib.dp_oracle_align.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
         lib.dp_oracle_construct.argtypes = [vp, vp, vp, u32, vp, vp, vp, vp, vp, vp, vp]
         _oracle = lib
@@ -121,6 +124,38 @@ def lcs_triangle(codes, offsets, lens, row_begin=0, row_end=None) -> np.ndarray:
 def transform(kind: int, lcs: int, len1: int, len2: int, double=True) -> float:
     lib = oracle()
     return float((lib.lcs_oracle_transform_f64 if double else lib.lcs_oracle_transform_f32)(kind, lcs, len1, len2))
+
+
+def transform_triangle(kind: int, lcs_tri: np.ndarray, lens) -> np.ndarray:
+    """transform(kind, ..., double=False) of every pair of a packed LCS triangle (uint16 or uint32, row i at i(i-1)/2,
+    row i = seq0): the float distance triangle UPGMA's computeDistances fills."""
+    t = np.ascontiguousarray(lcs_tri)
+    if t.dtype not in (np.uint16, np.uint32):
+        t = t.astype(np.uint32)
+    ln = np.ascontiguousarray(lens, dtype=np.uint32)
+    n = len(ln)
+    assert t.size == n * (n - 1) // 2
+    out = np.empty(max(t.size, 1), dtype=np.float32)
+    oracle().lcs_oracle_transform_tri_f32(kind, _p(t), t.dtype.itemsize, _p(ln), n, _p(out))
+    return out[:t.size]
+
+
+UPGMA_AVG_AS_REFERENCE, UPGMA_AVG_ROUNDED_ONCE, UPGMA_AVG_FUSED = 0, 1, 2
+
+
+def upgma_tree(dist_tri: np.ndarray, n: int, modified: bool = False, avg_mode: int = UPGMA_AVG_AS_REFERENCE,
+               fresh_cache: bool = False, overwrite: bool = False):
+    """The restated UPGMA<>::computeTree (oracle/upgma_oracle.c) on a float distance triangle, left untouched unless
+    `overwrite` (then a float32 array is averaged in place, as the reference does, which saves a copy of a large one).
+    Returns (status, merges): status 0 with the n-1 merges as (n-1, 2) int32, or 1 (no finite distance left) with the
+    merges made before that.  avg_mode / fresh_cache select the variants that only witness generation uses."""
+    ok_in_place = overwrite and isinstance(dist_tri, np.ndarray) and dist_tri.dtype == np.float32 and dist_tri.flags.c_contiguous
+    d = dist_tri if ok_in_place else np.array(dist_tri, dtype=np.float32, copy=True)
+    assert d.size == n * (n - 1) // 2
+    out = np.zeros((max(n - 1, 1), 2), dtype=np.int32)
+    done = C.c_uint32()
+    rc = oracle().upgma_oracle_tree(_p(d), n, int(modified), avg_mode, int(fresh_cache), _p(out), C.byref(done))
+    return rc, out[:done.value]
 
 
 # ------------------------------------------------------------------ the real reference

@@ -189,8 +189,12 @@ def rejected(eng, n):
             ("assign_shard seed >= n", lcs_calls(eng, n, d_out=d, seed=big)["assign_shard"]),
             ("upgma tree NULL", lambda: lib.famsa_lcs_upgma(h, 0, 0, NULL)),
             ("upgma kind 3", lcs_calls(eng, n, kind=3)["upgma"]),
+            ("upgma kind 2", lcs_calls(eng, n, kind=2)["upgma"]),                  # a similarity: no UPGMA instantiation
+            ("upgma kind -1", lcs_calls(eng, n, kind=-1)["upgma"]),
             ("upgma_from_triangle NULL", lcs_calls(eng, n)["upgma_from_triangle"]),
             ("upgma_from_triangle kind -1", lcs_calls(eng, n, kind=-1, d_out=d)["upgma_from_triangle"]),
+            ("upgma_from_triangle kind 2", lcs_calls(eng, n, kind=2, d_out=d)["upgma_from_triangle"]),
+            ("upgma_from_triangle kind 3", lcs_calls(eng, n, kind=3, d_out=d)["upgma_from_triangle"]),
             ("dist_export kind 2", lcs_calls(eng, n, kind=2)["dist_export"]),
             ("dist_export ids NULL", lambda: lib.famsa_dist_export(h, 0, 0, 0, NULL, vp(export_args(n)[1]), 0, SINK, NULL, NULL)),
             ("dist_export decreasing offsets", lambda: lib.famsa_dist_export(h, 0, 0, 1, export_args(n)[0],
