@@ -9,8 +9,31 @@
 #include <vector>
 
 #include "ctx.h"
+#include "triangle_dev.cuh"
 
 namespace fb {
+int DevBuf::reserve(size_t bytes)
+{
+    if (bytes <= cap) return FAMSA_OK;
+    release();
+    size_t want = bytes + bytes / 8 + 256;
+    cudaError_t e = cudaMalloc(&p, want);
+    if (e != cudaSuccess) {
+        p = nullptr;
+        cudaGetLastError();          // callers may recover (famsa_lcs_prim falls back): do not leave the error for a later check
+        set_error(std::string("cudaMalloc(") + std::to_string(want) + ") failed: " + cudaGetErrorString(e));
+        return FAMSA_E_NOMEM;
+    }
+    cap = want;
+    return FAMSA_OK;
+}
+void DevBuf::release()
+{
+    if (p) cudaFree(p);
+    p = nullptr;
+    cap = 0;
+}
+
 static thread_local std::string g_error;
 void set_error(const std::string& msg) { g_error = msg; }
 const char* get_error() { return g_error.c_str(); }
@@ -30,6 +53,7 @@ int scratch_release(famsa_ctx* ctx, cudaStream_t st, bool synced)
 } // namespace fb
 
 using fb::set_error;
+using fb::tri_index;
 
 #define FB_CHECK_CTX(ctx)                          \
     if (!(ctx)) {                                  \
@@ -112,8 +136,6 @@ static int check_ids(const famsa_ctx* ctx, const uint32_t* ids, uint32_t count, 
         if (ids[k] >= ctx->lcs.n) { set_error(std::string(what) + " id out of range"); return FAMSA_E_INVALID; }
     return FAMSA_OK;
 }
-
-static uint64_t tri(uint64_t r) { return r ? r * (r - 1) / 2 : 0; }
 
 extern "C" {
 
@@ -262,14 +284,14 @@ int famsa_lcs_triangle_device(famsa_ctx* ctx, uint32_t row_begin, uint32_t row_e
         if (!d_out && row_end > row_begin && row_end > 1) { set_error("d_out is NULL"); return FAMSA_E_INVALID; }
         return FAMSA_OK;
     }, [&](cudaStream_t st) -> int {
-        ctx->lcs.last_pairs = tri(row_end) - tri(row_begin);
+        ctx->lcs.last_pairs = tri_index(row_end, 0) - tri_index(row_begin, 0);
         return lcs_timed(ctx, st, [&] { return fb::lcs_triangle(ctx, row_begin, row_end, d_out, elem_bytes, st); });
     });
 }
 
 int famsa_lcs_triangle(famsa_ctx* ctx, uint32_t row_begin, uint32_t row_end, void* out, int elem_bytes)
 {
-    const uint64_t pairs = tri(row_end) - tri(row_begin);
+    const uint64_t pairs = tri_index(row_end, 0) - tri_index(row_begin, 0);
     return entry(ctx, nullptr, nullptr, [&]() -> int {
         FB_TRY(check_rows(ctx, row_begin, row_end));
         FB_TRY(check_elem(elem_bytes, ctx->lcs.elem_bytes()));
@@ -293,8 +315,8 @@ int famsa_lcs_triangle(famsa_ctx* ctx, uint32_t row_begin, uint32_t row_end, voi
         if (!S.identity_perm && n_blocks == 1) FB_CUDA(cudaEventRecord(ctx->ev_block[0], st));
         FB_CUDA(cudaEventRecord(ctx->ev_host[1], st));
         for (int b = 0; b < n_blocks; ++b) {
-            const uint64_t off = (tri(bounds[b]) - tri(row_begin)) * elem_bytes;
-            const uint64_t bytes = (tri(bounds[b + 1]) - tri(bounds[b])) * elem_bytes;
+            const uint64_t off = (tri_index(bounds[b], 0) - tri_index(row_begin, 0)) * elem_bytes;
+            const uint64_t bytes = (tri_index(bounds[b + 1], 0) - tri_index(bounds[b], 0)) * elem_bytes;
             if (!bytes) continue;
             FB_CUDA(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_block[b], 0));
             FB_CUDA(cudaMemcpyAsync(static_cast<char*>(out) + off, d_out + off, bytes, cudaMemcpyDeviceToHost, ctx->copy_stream));
@@ -384,8 +406,8 @@ int famsa_lcs_triangle_exchange(famsa_ctx* ctx, uint32_t row_begin, uint32_t row
         for (uint32_t b = 0; b <= np; ++b) frac[b] = np == 8 ? kCut8[b] : (double)b / np;
         uint32_t bounds[kPieces + 1];
         fb::lcs_row_pieces(row_begin, row_end, (int)np, frac, bounds);
-        ctx->lcs.last_pairs = tri(row_end) - tri(row_begin);
-        char* own = static_cast<char*>(d_full) + tri(row_begin) * elem_bytes;    // lcs_triangle indexes from its first row
+        ctx->lcs.last_pairs = tri_index(row_end, 0) - tri_index(row_begin, 0);
+        char* own = static_cast<char*>(d_full) + tri_index(row_begin, 0) * elem_bytes;    // lcs_triangle indexes from its first row
         FB_TRY(lcs_timed(ctx, st, [&] {
             return fb::lcs_triangle(ctx, row_begin, row_end, own, elem_bytes, st, bounds, (int)np, ctx->ev_block, true, true);
         }));
@@ -401,7 +423,7 @@ int famsa_lcs_triangle_exchange(famsa_ctx* ctx, uint32_t row_begin, uint32_t row
         }
         const int n_lanes = (int)std::min<uint32_t>(n_peers, kLanes);
         for (uint32_t b = 0; b < np; ++b) {
-            const uint64_t off = tri(bounds[b]) * elem_bytes, bytes = (tri(bounds[b + 1]) - tri(bounds[b])) * elem_bytes;
+            const uint64_t off = tri_index(bounds[b], 0) * elem_bytes, bytes = (tri_index(bounds[b + 1], 0) - tri_index(bounds[b], 0)) * elem_bytes;
             if (!bytes) continue;
             for (int a = 0; a < n_lanes; ++a) FB_CUDA(cudaStreamWaitEvent(lanes[a], ctx->ev_block[b], 0));
             for (uint32_t k = 0; k < n_peers; ++k)
@@ -475,7 +497,7 @@ int famsa_lcs_prim(famsa_ctx* ctx, int distance_kind, int32_t* edge_from, int32_
         if (distance_kind != 0 && distance_kind != 1) { set_error("MSTPrim is instantiated for distance_kind 0 and 1 only"); return FAMSA_E_INVALID; }
         return FAMSA_OK;
     }, [&](cudaStream_t st) -> int {
-        ctx->lcs.last_pairs = tri(ctx->lcs.n);
+        ctx->lcs.last_pairs = tri_index(ctx->lcs.n, 0);
         return lcs_timed(ctx, st, [&] { return fb::lcs_prim(ctx, distance_kind, edge_from, edge_to, edge_dist, prim_order, tree); });
     });
     if (rc || tree.empty()) return rc;
@@ -491,7 +513,7 @@ int famsa_lcs_slink(famsa_ctx* ctx, int distance_kind, int32_t* tree)
         if (distance_kind != 0 && distance_kind != 1) { set_error("SingleLinkage is instantiated for distance_kind 0 and 1 only"); return FAMSA_E_INVALID; }
         return FAMSA_OK;
     }, [&](cudaStream_t st) -> int {
-        ctx->lcs.last_pairs = tri(ctx->lcs.n);
+        ctx->lcs.last_pairs = tri_index(ctx->lcs.n, 0);
         return lcs_timed(ctx, st, [&] { return fb::lcs_slink(ctx, distance_kind, edges); });
     });
     if (rc || edges.empty()) return rc;
@@ -522,7 +544,7 @@ int famsa_lcs_upgma(famsa_ctx* ctx, int distance_kind, int modified, int32_t* tr
         if (distance_kind != 0 && distance_kind != 1) { set_error("UPGMA is instantiated for distance_kind 0 and 1 only"); return FAMSA_E_INVALID; }
         return FAMSA_OK;
     }, [&](cudaStream_t st) -> int {
-        ctx->lcs.last_pairs = tri(ctx->lcs.n);
+        ctx->lcs.last_pairs = tri_index(ctx->lcs.n, 0);
         return lcs_timed(ctx, st, [&] { return fb::lcs_upgma(ctx, distance_kind, modified, tree); });
     });
 }

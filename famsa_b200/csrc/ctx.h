@@ -73,7 +73,7 @@ struct LcsState {
     // element width that holds every LCS of the set: u16 while every sequence is shorter than 65536 residues
     int elem_bytes() const { return max_len < 65536 ? 2 : 4; }
     DevBuf d_perm, d_invperm, d_len_sorted, d_code_off, d_codes, d_blob, d_group_blob;
-    DevBuf d_raw_codes, d_raw_off, d_raw_len, d_flags, d_pow075, d_pow075_f64, d_assign_lcs, d_assign, d_mind;
+    DevBuf d_raw_codes, d_raw_off, d_raw_len, d_flags, d_pow075, d_pow075_f64, d_assign_lcs;
     // the guide trees and the export
     DevBuf d_lcs_tri;                        // resident LCS triangle (prim, UPGMA, export), elem_bytes() wide
     DevBuf d_dist_tri;                       // distance triangle: float64 for the Boruvka rounds, float32 for UPGMA
@@ -249,7 +249,7 @@ struct famsa_ctx {
 };
 
 namespace fb {
-// capi.cu: ordering of calls that share the context's scratch
+// capi.cu: ordering of calls that share the context's scratch (DevBuf::reserve/release live there too)
 int scratch_acquire(famsa_ctx* ctx, cudaStream_t st);   // call before queueing work that uses the scratch on `st`
 int scratch_release(famsa_ctx* ctx, cudaStream_t st, bool synced);   // call after queueing (synced: the stream was synchronised)
 // lcs.cu
@@ -264,7 +264,13 @@ void lcs_row_pieces(uint32_t row_begin, uint32_t row_end, int n_pieces, const do
 int lcs_rows(famsa_ctx* ctx, const uint32_t* h_ref_ids, uint32_t n_ref, const uint32_t* d_col_ids, uint32_t n_col, void* d_out,
              int elem_bytes, cudaStream_t stream, uint32_t g_begin = 0, uint32_t g_end = 0xffffffffu);
 int lcs_side_rows(famsa_ctx* ctx, cudaStream_t st);
+int lcs_pow075_f64(famsa_ctx* ctx, cudaStream_t st);
+int lcs_exact_block(famsa_ctx* ctx, const std::vector<uint32_t>& rows, const uint32_t* d_col_ids, uint32_t n_col, void* d_out,
+                    int elem_bytes, cudaStream_t st);
+// tree.cu
 int lcs_upgma(famsa_ctx* ctx, int kind, int modified, int32_t* h_tree, const void* d_tri_in = nullptr, int tri_eb = 2);
+int lcs_assign(famsa_ctx* ctx, const uint32_t* h_seed_ids, uint32_t n_seeds, int kind, uint32_t* h_assign,
+               float* h_mind);
 int lcs_assign_shard(famsa_ctx* ctx, const uint32_t* h_seed_ids, uint32_t n_seeds, int kind, uint32_t shard, uint32_t n_shards,
                      long long* d_packed, cudaStream_t st);
 struct MstEdge { uint32_t a, b; double d; };
@@ -275,11 +281,6 @@ int prim_replay(const std::vector<MstEdge>& tree, int32_t* h_from, int32_t* h_to
 // SLINK's MST into `edges` (either engine); slink_labels (host only) turns it into the n-1 merges of SLINK's tree
 int lcs_slink(famsa_ctx* ctx, int kind, std::vector<MstEdge>& edges);
 void slink_labels(std::vector<MstEdge> edges, uint32_t n, int32_t* tree);
-int lcs_assign(famsa_ctx* ctx, const uint32_t* h_seed_ids, uint32_t n_seeds, int kind, uint32_t* h_assign,
-               float* h_mind);
-int lcs_pow075_f64(famsa_ctx* ctx, cudaStream_t st);
-int lcs_exact_block(famsa_ctx* ctx, const std::vector<uint32_t>& rows, const uint32_t* d_col_ids, uint32_t n_col, void* d_out,
-                    int elem_bytes, cudaStream_t st);
 // dist_export.cu
 int dist_export(famsa_ctx* ctx, int kind, int square, int pid, const char* ids, const uint64_t* id_offsets,
                 uint64_t chunk_bytes, famsa_write_fn write, void* user, uint64_t* bytes_written);

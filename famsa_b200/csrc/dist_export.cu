@@ -13,7 +13,6 @@
 //     chunks and prefix-sums the row offsets; pass 2, one block per row, formats 1024 values at a time: per-value
 //     lengths, a block scan, the characters into shared memory at the destination's 16-byte phase, then aligned 16-byte
 //     stores (bytes at the two ragged ends).  Every byte has one writer and one value, so the text is deterministic.
-#include <cfloat>
 #include <cmath>
 #include <cstring>
 #include <string>
@@ -23,7 +22,7 @@
 #include <cub/block/block_scan.cuh>
 
 #include "ctx.h"
-#include "transform_dev.cuh"
+#include "triangle_dev.cuh"
 
 namespace fb {
 
@@ -39,7 +38,6 @@ struct DistParams {
     uint32_t n;
     const uint32_t* lens;          // caller order
     const double* pow075;          // (double) pow(i, 0.75), host libm
-    double never;                  // nextafter(DBL_MAX, 0)
     int kind, pid, square;
     const int* side_idx;           // square: row of a flagged sequence in `side` / column in `colq`, else -1
     const uint32_t* side;          // nq x n: flagged sequence as seq0 against every column
@@ -107,8 +105,7 @@ __device__ __forceinline__ void put_value(char* dst, unsigned long long a, unsig
 
 __device__ __forceinline__ uint32_t tri_at(const DistParams& P, uint32_t i, uint32_t j)          // i > j
 {
-    const size_t at = (size_t)i * (i - 1) / 2 + j;
-    return P.eb == 2 ? static_cast<const uint16_t*>(P.tri)[at] : static_cast<const uint32_t*>(P.tri)[at];
+    return lcs_load(P.tri, P.eb, tri_index(i, j));
 }
 
 // LCS with r as seq0 and c streamed (c < r in triangle mode)
@@ -129,8 +126,8 @@ __device__ __forceinline__ uint32_t cell_lcs(const DistParams& P, uint32_t r, ui
 __device__ __forceinline__ float cell_value(const DistParams& P, uint32_t r, uint32_t c)
 {
     const uint32_t lcs = cell_lcs(P, r, c);
-    if (P.pid) return transform_f32(2, lcs, P.lens[r], P.lens[c], nullptr, 0.f);
-    return __double2float_rn(transform_f64(P.kind, lcs, P.lens[r], P.lens[c], P.pow075, P.never));
+    if (P.pid) return transform_f32(2, lcs, P.lens[r], P.lens[c], nullptr);
+    return __double2float_rn(transform_f64(P.kind, lcs, P.lens[r], P.lens[c], P.pow075));
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -260,7 +257,7 @@ int dist_export(famsa_ctx* ctx, int kind, int square, int pid, const char* ids, 
     cudaStream_t st = ctx->stream;
     const uint32_t n = S.n;
     const int eb = S.elem_bytes();
-    const uint64_t pairs = (uint64_t)n * (n - 1) / 2;
+    const uint64_t pairs = tri_index(n, 0);
     uint64_t written = 0;
     if (bytes_written) *bytes_written = 0;
     if (!S.ev_dx[0])
@@ -314,7 +311,6 @@ int dist_export(famsa_ctx* ctx, int kind, int square, int pid, const char* ids, 
     P.tri = S.d_lcs_tri.p; P.eb = eb; P.n = n;
     P.lens = S.d_raw_len.as<uint32_t>();
     P.pow075 = S.d_pow075_f64.as<double>();
-    P.never = nextafter(DBL_MAX, 0.0);
     P.kind = kind; P.pid = pid; P.square = square;
     P.side_idx = S.d_side_idx.as<int>(); P.side = S.d_side_rows.as<uint32_t>(); P.colq = S.d_dx_colq.as<uint32_t>(); P.nq = nq;
     P.diag = d_diag;

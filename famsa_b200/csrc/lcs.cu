@@ -23,17 +23,12 @@
 //     k_lcs_exact, which follows the reference recurrence word for word.
 #include <algorithm>
 #include <atomic>
-#include <cfloat>
 #include <cmath>
 #include <cstring>
 #include <numeric>
-#include <queue>
-#include <tuple>
-
-#include <cooperative_groups.h>
 
 #include "ctx.h"
-#include "transform_dev.cuh"
+#include "triangle_dev.cuh"
 
 namespace fb {
 
@@ -309,17 +304,11 @@ __global__ void __launch_bounds__(kTileWarps * 32) k_lcs_tile(const TileParams P
         for (int w = 0; w < NL; ++w) lcs += __popc(~X[w]);
 
         if (P.rows_mode) {
-            const size_t idx = (size_t)q * P.ld_res + p;
-            if (P.elem_bytes == 2) static_cast<uint16_t*>(P.out)[idx] = (uint16_t)lcs;
-            else static_cast<uint32_t*>(P.out)[idx] = lcs;
+            lcs_store(P.out, P.elem_bytes, (size_t)q * P.ld_res + p, lcs);
         } else if (a != 0xffffffffu && sq < p) {
             const uint32_t b = P.perm[sq];
             const uint32_t i = a > b ? a : b, j = a > b ? b : a;
-            if (i >= P.row_begin && i < P.row_end) {
-                const size_t idx = (size_t)i * (i - 1) / 2 - P.tri_base + j;
-                if (P.elem_bytes == 2) static_cast<uint16_t*>(P.out)[idx] = (uint16_t)lcs;
-                else static_cast<uint32_t*>(P.out)[idx] = lcs;
-            }
+            if (i >= P.row_begin && i < P.row_end) lcs_store(P.out, P.elem_bytes, tri_index(i, 0) - P.tri_base + j, lcs);
         }
     }
 }
@@ -333,12 +322,8 @@ __global__ void k_gather_rows(const void* __restrict__ res, uint32_t ld_res, int
     const uint32_t r = blockIdx.y;
     if (k >= n_col) return;
     const uint32_t c = col_ids ? col_ids[k] : k;
-    const size_t src = (size_t)r * ld_res + invperm[c];
-    const uint32_t v = res_bytes == 2 ? static_cast<const uint16_t*>(res)[src]
-                                      : static_cast<const uint32_t*>(res)[src];
-    const size_t dst = (size_t)r * n_col + k;
-    if (elem_bytes == 2) static_cast<uint16_t*>(out)[dst] = (uint16_t)v;
-    else static_cast<uint32_t*>(out)[dst] = v;
+    const uint32_t v = lcs_load(res, res_bytes, (size_t)r * ld_res + invperm[c]);
+    lcs_store(out, elem_bytes, (size_t)r * n_col + k, v);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -398,9 +383,7 @@ __global__ void k_lcs_exact(const uint8_t* __restrict__ codes, const uint32_t* _
     }
     uint32_t lcs = 0;
     for (uint32_t w = 0; w < nw; ++w) lcs += __popcll(~x[w * stride]);
-    const size_t idx = out_base + k;
-    if (elem_bytes == 2) static_cast<uint16_t*>(out)[idx] = (uint16_t)lcs;
-    else static_cast<uint32_t*>(out)[idx] = lcs;
+    lcs_store(out, elem_bytes, out_base + k, lcs);
 }
 
 // All special rows of a call in ONE launch: blockIdx.y = the row, its 64-bit masks are built in shared memory by the
@@ -449,507 +432,23 @@ __global__ void __launch_bounds__(128) k_lcs_exact_batch(const uint8_t* __restri
     }
     uint32_t lcs = 0;
     for (uint32_t w = 0; w < nw; ++w) lcs += __popcll(~x[w]);
-    const size_t idx = R.out_base + k;
-    if (elem_bytes == 2) static_cast<uint16_t*>(out)[idx] = (uint16_t)lcs;
-    else static_cast<uint32_t*>(out)[idx] = lcs;
-}
-
-// ------------------------------------------------------------------------------------------------
-// medoid assignment: float Transform + running arg-min over the seed rows (FastTree.cpp:309-324)
-// ------------------------------------------------------------------------------------------------
-
-// transform_f32 / transform_f64 (Transform<float|double, Distance>): transform_dev.cuh
-
-__global__ void k_assign(const void* __restrict__ lcs, int elem_bytes, uint32_t n, uint32_t n_seeds,
-                         const uint32_t* __restrict__ seed_ids, const uint32_t* __restrict__ lens,
-                         const float* __restrict__ pow075, int kind, float never,
-                         uint32_t* __restrict__ assign, float* __restrict__ mind)
-{
-    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= n) return;
-    const uint32_t lj = lens[j];
-    float best = 0.f;
-    uint32_t a = 0;
-    for (uint32_t k = 0; k < n_seeds; ++k) {
-        const size_t at = (size_t)k * n + j;
-        const uint32_t l = elem_bytes == 2 ? static_cast<const uint16_t*>(lcs)[at] : static_cast<const uint32_t*>(lcs)[at];
-        const float d = transform_f32(kind, l, lens[seed_ids[k]], lj, pow075, never);
-        if (k == 0 || d < best) { best = d; a = k; }
-    }
-    assign[j] = a;
-    mind[j] = best;
-}
-
-// Sharded form: only the sequences whose mask group lies in [g_begin, g_end) are answered; the result is packed as
-// (float bits of the distance << 32) | seed index so that an element-wise MIN over the shards (one all-reduce) assembles
-// the complete assignment -- distances are >= 0, so their bit patterns order like the values, and among equal distances
-// the lowest seed index wins, which is what the strict < of the sequential loop does.  Unanswered entries hold INT64_MAX.
-__global__ void k_assign_packed(const void* __restrict__ lcs, int elem_bytes, uint32_t n, uint32_t n_seeds,
-                                const uint32_t* __restrict__ seed_ids, const uint32_t* __restrict__ lens,
-                                const float* __restrict__ pow075, int kind, float never,
-                                const uint32_t* __restrict__ invperm, uint32_t g_begin, uint32_t g_end,
-                                long long* __restrict__ packed)
-{
-    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= n) return;
-    const uint32_t g = invperm[j] / 32;
-    if (g < g_begin || g >= g_end) { packed[j] = 0x7fffffffffffffffll; return; }
-    const uint32_t lj = lens[j];
-    float best = 0.f;
-    uint32_t a = 0;
-    for (uint32_t k = 0; k < n_seeds; ++k) {
-        const size_t at = (size_t)k * n + j;
-        const uint32_t l = elem_bytes == 2 ? static_cast<const uint16_t*>(lcs)[at] : static_cast<const uint32_t*>(lcs)[at];
-        const float d = transform_f32(kind, l, lens[seed_ids[k]], lj, pow075, never);
-        if (k == 0 || d < best) { best = d; a = k; }
-    }
-    packed[j] = (long long)(((unsigned long long)__float_as_uint(best) << 32) | a);
-}
-
-// ------------------------------------------------------------------------------------------------
-// MST-Prim vertex loop (MSTPrim<>::run_view, MSTPrim.cpp:280-549) on the resident LCS triangle
-// ------------------------------------------------------------------------------------------------
-
-struct PrimState {                 // per sequence: best known connection to the tree
-    double dist;
-    unsigned long long key;        // ~ids_to_uint64(from, j)  (MSTPrim.h:432-439)
-};
-
-// Cooperative grid (one block per SM, all co-resident): per step every thread relaxes its own unvisited sequences
-// against the current vertex (one triangle lookup + one pow-table lookup each, all independent), blocks publish their
-// best (dist, key) pair, ONE grid-wide barrier, and every block reduces the published candidates itself, so all
-// blocks agree on the next vertex without a second barrier.  Candidate slots are double-buffered by step parity.
-// tri: true-LCS triangle in caller order; side rows hold the row-oriented values of the sequences whose LCS is
-// orientation dependent (dropped-carry corner): side_idx[v] = row in `side` or -1.
-// kSlink (famsa_lcs_slink): tri is the triangle SLINK reads (row = seq0, dropped-carry rows exact), every lookup reads
-// it (side_idx and side are not read), and there is no lower-bound skip -- SingleLinkage has none.
-struct PrimCand {
-    double dist;
-    unsigned long long key;
-    int id;
-    int pad;
-};
-
-template <bool kSlink>
-__global__ void __launch_bounds__(1024) k_prim(const void* __restrict__ tri, int eb, uint32_t n,
-                                               const uint32_t* __restrict__ lens, const double* __restrict__ pow075,
-                                               int kind, double never, const int* __restrict__ side_idx,
-                                               const uint32_t* __restrict__ side, PrimState* __restrict__ st,
-                                               unsigned char* __restrict__ visited, PrimCand* __restrict__ cand,
-                                               int* __restrict__ out_from, int* __restrict__ out_to,
-                                               double* __restrict__ out_dist, int* __restrict__ order)
-{
-    namespace cg = cooperative_groups;
-    cg::grid_group grid = cg::this_grid();
-    __shared__ double sh_d[32];
-    __shared__ unsigned long long sh_k[32];
-    __shared__ int sh_id[32];
-    __shared__ int sh_v;
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t gtid = blockIdx.x * blockDim.x + tid, gthreads = gridDim.x * blockDim.x;
-    const uint32_t nblk = gridDim.x;
-    auto better = [](double d, unsigned long long k, int id, double bd, unsigned long long bk, int bid) {
-        return id >= 0 && (bid < 0 || d < bd || (d == bd && k < bk));
-    };
-    for (uint32_t j = gtid; j < n; j += gthreads) {
-        st[j].dist = 1.7976931348623157e308;        // numeric_limits<double>::max()
-        st[j].key = 0;
-        visited[j] = j == 0;
-        order[j] = j == 0 ? 0 : (int)n;
-    }
-    // the first sequence a thread owns lives in registers (with n <= gridDim.x * 1024 that is all of them)
-    const bool has0 = gtid < n;
-    const uint32_t len0 = has0 ? lens[gtid] : 0;
-    bool vis0 = gtid == 0;
-    double d0 = 1.7976931348623157e308;
-    unsigned long long k0 = 0;
-    uint32_t v = 0;
-    grid.sync();
-    for (uint32_t step = 1; step < n; ++step) {
-        const uint32_t lv = lens[v];
-        const int sv = kSlink ? -1 : side_idx[v];
-        double bd = 0.0;
-        unsigned long long bk = 0;
-        int bid = -1;
-        auto lookup = [&](uint32_t j) -> uint32_t {
-            if (sv >= 0) return side[(size_t)sv * n + j];
-            const uint32_t hi = v > j ? v : j, lo = v > j ? j : v;
-            const size_t at = (size_t)hi * (hi - 1) / 2 + lo;
-            return eb == 2 ? static_cast<const uint16_t*>(tri)[at] : static_cast<const uint32_t*>(tri)[at];
-        };
-        // MSTPrim.cpp:450-467: a candidate is only computed when the distance it would have with LCS = the shorter length
-        // does not exceed its current one.  A no-op for a true LCS (<= the shorter length); with the dropped-carry corner the
-        // reference's LCS can be larger, and then the skip decides whether the candidate is relaxed.
-        if (has0 && !vis0) {
-            const uint32_t j = gtid;
-            const bool tried = kSlink || transform_f64(kind, lv < len0 ? lv : len0, lv, len0, pow075, never) <= d0;
-            const double d = tried ? transform_f64(kind, lookup(j), lv, len0, pow075, never) : 1.7976931348623157e308;
-            if (tried && d <= d0) {
-                const unsigned long long a = v < j ? v : j, b = v < j ? j : v;
-                const unsigned long long k = ~((a << 32) + b);
-                if (d < d0 || k < k0) { d0 = d; k0 = k; }                                  // pair <, given d <= d0
-            }
-            bd = d0; bk = k0; bid = (int)j;
-        }
-        for (uint32_t j = gtid + gthreads; j < n; j += gthreads) {                         // only when n > grid size
-            if (visited[j]) continue;
-            double cd = st[j].dist;
-            unsigned long long ck = st[j].key;
-            const uint32_t lj = lens[j];
-            const bool tried = kSlink || transform_f64(kind, lv < lj ? lv : lj, lv, lj, pow075, never) <= cd;
-            const double d = tried ? transform_f64(kind, lookup(j), lv, lj, pow075, never) : 1.7976931348623157e308;
-            if (tried && d <= cd) {
-                const unsigned long long a = v < j ? v : j, b = v < j ? j : v;
-                const unsigned long long k = ~((a << 32) + b);
-                if (d < cd || k < ck) { cd = d; ck = k; st[j].dist = cd; st[j].key = ck; }
-            }
-            if (better(cd, ck, (int)j, bd, bk, bid)) { bd = cd; bk = ck; bid = (int)j; }
-        }
-        // block-wide minimum of (dist, key) ...
-        for (int o = 16; o; o >>= 1) {
-            const double od = __shfl_xor_sync(0xffffffffu, bd, o);
-            const unsigned long long ok = __shfl_xor_sync(0xffffffffu, bk, o);
-            const int oid = __shfl_xor_sync(0xffffffffu, bid, o);
-            if (better(od, ok, oid, bd, bk, bid)) { bd = od; bk = ok; bid = oid; }
-        }
-        if (lane == 0) { sh_d[warp] = bd; sh_k[warp] = bk; sh_id[warp] = bid; }
-        __syncthreads();
-        if (warp == 0) {
-            const uint32_t nw = blockDim.x / 32;
-            bd = lane < nw ? sh_d[lane] : 0.0; bk = lane < nw ? sh_k[lane] : 0; bid = lane < nw ? sh_id[lane] : -1;
-            for (int o = 16; o; o >>= 1) {
-                const double od = __shfl_xor_sync(0xffffffffu, bd, o);
-                const unsigned long long ok = __shfl_xor_sync(0xffffffffu, bk, o);
-                const int oid = __shfl_xor_sync(0xffffffffu, bid, o);
-                if (better(od, ok, oid, bd, bk, bid)) { bd = od; bk = ok; bid = oid; }
-            }
-            if (lane == 0) {
-                PrimCand c; c.dist = bd; c.key = bk; c.id = bid; c.pad = 0;
-                cand[(step & 1) * nblk + blockIdx.x] = c;
-            }
-        }
-        // ... one grid barrier, then every block reduces the published candidates for itself
-        grid.sync();
-        if (warp == 0) {
-            bd = 0.0; bk = 0; bid = -1;
-            for (uint32_t b = lane; b < nblk; b += 32) {
-                const PrimCand c = cand[(step & 1) * nblk + b];
-                if (better(c.dist, c.key, c.id, bd, bk, bid)) { bd = c.dist; bk = c.key; bid = c.id; }
-            }
-            for (int o = 16; o; o >>= 1) {
-                const double od = __shfl_xor_sync(0xffffffffu, bd, o);
-                const unsigned long long ok = __shfl_xor_sync(0xffffffffu, bk, o);
-                const int oid = __shfl_xor_sync(0xffffffffu, bid, o);
-                if (better(od, ok, oid, bd, bk, bid)) { bd = od; bk = ok; bid = oid; }
-            }
-            if (lane == 0) {
-                sh_v = bid;
-                if (blockIdx.x == 0) {
-                    const unsigned long long packed = ~bk;             // uint64_to_id (MSTPrim.h:441-450)
-                    const int id1 = (int)(packed >> 32), id2 = (int)(packed & 0xffffffffull);
-                    out_from[step - 1] = id1 < id2 ? id1 : id2;
-                    out_to[step - 1] = id1 < id2 ? id2 : id1;
-                    out_dist[step - 1] = bd;
-                    order[bid] = (int)step;
-                }
-                if ((uint32_t)bid >= gthreads && (uint32_t)bid % gthreads / blockDim.x == blockIdx.x) visited[bid] = 1;   // its owner block
-            }
-        }
-        __syncthreads();
-        v = (uint32_t)sh_v;
-        if (v == gtid) vis0 = true;
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
-// Parallel MST (Boruvka rounds) under MSTPrim's edge order.
-//
-// MSTPrim relaxes and elects with the pair (distance, ~ids_to_uint64(min id, max id)) compared lexicographically
-// (MSTPrim.cpp:366-386, 492-503).  The key is unique per edge, so the pairs are a strict total order and the minimum
-// spanning tree under it is unique: any algorithm finds the edges Prim finds.  What Prim adds is the visiting order
-// from vertex 0, and that can be replayed on the n-1 tree edges alone (at every step Prim takes the smallest edge
-// leaving the visited set, which is a tree edge).  So: distances once into a float64 triangle, then log2(n) rounds in
-// which every vertex finds its smallest edge into another component -- two streaming passes over the triangle, rows
-// and columns, both coalesced -- while the host merges components (union-find over n entries) and finally replays
-// Prim's order with a heap.  Used when no sequence has orientation-dependent LCS values (the dropped-carry corner);
-// otherwise the sequential loop above runs.  famsa_b200/mst.py + tests/test_mst_host.py pin the argument on the CPU.
-// ------------------------------------------------------------------------------------------------
-struct EdgeMin {
-    double d;
-    unsigned long long k;
-};
-__device__ __forceinline__ bool edge_less(double d, unsigned long long k, double bd, unsigned long long bk) { return d < bd || (d == bd && k < bk); }
-__device__ __forceinline__ unsigned long long edge_key_dev(uint32_t a, uint32_t b)
-{
-    const unsigned long long lo = a < b ? a : b, hi = a < b ? b : a;
-    return ~((lo << 32) + hi);
-}
-constexpr double kEdgeNone = __builtin_huge_val();      // +inf: no candidate (distances are finite)
-
-// one block per row i: distances of (i, j), j < i  (Transform<double, Distance>, AbstractTreeGenerator.hpp:28-82)
-__global__ void __launch_bounds__(256) k_mst_dist(const void* __restrict__ tri, int eb, uint32_t n, const uint32_t* __restrict__ lens,
-                                                  const double* __restrict__ pow075, int kind, double never, double* __restrict__ out)
-{
-    const uint32_t i = blockIdx.x + 1;
-    const size_t base = (size_t)i * (i - 1) / 2;
-    const uint32_t li = lens[i];
-    for (uint32_t j = threadIdx.x; j < i; j += blockDim.x) {
-        const uint32_t l = eb == 2 ? static_cast<const uint16_t*>(tri)[base + j] : static_cast<const uint32_t*>(tri)[base + j];
-        out[base + j] = transform_f64(kind, l, li, lens[j], pow075, never);
-    }
-}
-
-__device__ __forceinline__ void block_edge_min(double& d, unsigned long long& k)
-{
-    __shared__ double sd[32];
-    __shared__ unsigned long long sk[32];
-    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int o = 16; o; o >>= 1) {
-        const double od = __shfl_xor_sync(0xffffffffu, d, o);
-        const unsigned long long ok = __shfl_xor_sync(0xffffffffu, k, o);
-        if (edge_less(od, ok, d, k)) { d = od; k = ok; }
-    }
-    if (lane == 0) { sd[warp] = d; sk[warp] = k; }
-    __syncthreads();
-    if (warp == 0) {
-        const uint32_t nw = blockDim.x / 32;
-        d = lane < nw ? sd[lane] : kEdgeNone; k = lane < nw ? sk[lane] : 0;
-        for (int o = 16; o; o >>= 1) {
-            const double od = __shfl_xor_sync(0xffffffffu, d, o);
-            const unsigned long long ok = __shfl_xor_sync(0xffffffffu, k, o);
-            if (edge_less(od, ok, d, k)) { d = od; k = ok; }
-        }
-    }
-}
-
-// row pass: vertex i against its lower neighbours j < i in other components
-__global__ void __launch_bounds__(256) k_mst_rows(const double* __restrict__ dtri, uint32_t n, const uint32_t* __restrict__ comp,
-                                                  EdgeMin* __restrict__ best)
-{
-    const uint32_t i = blockIdx.x;
-    const size_t base = (size_t)i * (i ? i - 1 : 0) / 2;
-    const uint32_t ci = comp[i];
-    double d = kEdgeNone;
-    unsigned long long k = 0;
-    for (uint32_t j = threadIdx.x; j < i; j += blockDim.x) {
-        if (comp[j] == ci) continue;
-        const double dj = dtri[base + j];
-        const unsigned long long kj = edge_key_dev(i, j);
-        if (edge_less(dj, kj, d, k)) { d = dj; k = kj; }
-    }
-    block_edge_min(d, k);
-    if (threadIdx.x == 0) { best[i].d = d; best[i].k = k; }
-}
-
-// column pass: vertex j against its upper neighbours i > j; block = 32 columns x a chunk of kMstChunk rows, every row
-// contributes a coalesced 256-byte segment.  part[chunk][j] receives the chunk's minimum.
-constexpr uint32_t kMstChunk = 1024;
-__global__ void __launch_bounds__(256) k_mst_cols(const double* __restrict__ dtri, uint32_t n, const uint32_t* __restrict__ comp,
-                                                  EdgeMin* __restrict__ part)
-{
-    __shared__ double sd[8][32];
-    __shared__ unsigned long long sk[8][32];
-    const uint32_t x = threadIdx.x & 31, y = threadIdx.x >> 5;
-    const uint32_t j = blockIdx.x * 32 + x;
-    const uint32_t r0 = blockIdx.y * kMstChunk, r1 = r0 + kMstChunk < n ? r0 + kMstChunk : n;
-    double d = kEdgeNone;
-    unsigned long long k = 0;
-    if (j < n) {
-        const uint32_t cj = comp[j];
-        uint32_t i = r0 + y;
-        if (i <= j) i += ((j + 1 - i) + 7) / 8 * 8;                 // first row of this thread's residue class above j
-        for (; i < r1; i += 8) {
-            if (comp[i] == cj) continue;
-            const double di = dtri[(size_t)i * (i - 1) / 2 + j];
-            const unsigned long long ki = edge_key_dev(i, j);
-            if (edge_less(di, ki, d, k)) { d = di; k = ki; }
-        }
-    }
-    sd[y][x] = d; sk[y][x] = k;
-    __syncthreads();
-    if (y == 0 && j < n) {
-        for (int q = 1; q < 8; ++q)
-            if (edge_less(sd[q][x], sk[q][x], d, k)) { d = sd[q][x]; k = sk[q][x]; }
-        part[(size_t)blockIdx.y * n + j].d = d;
-        part[(size_t)blockIdx.y * n + j].k = k;
-    }
-}
-
-// best[j] = min(best[j] (row pass), part[*][j])
-__global__ void __launch_bounds__(256) k_mst_combine(uint32_t n, uint32_t n_chunks, const EdgeMin* __restrict__ part, EdgeMin* __restrict__ best)
-{
-    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= n) return;
-    double d = best[j].d;
-    unsigned long long k = best[j].k;
-    for (uint32_t c = j / kMstChunk; c < n_chunks; ++c) {            // chunks that end at or below row j hold nothing for j
-        const EdgeMin e = part[(size_t)c * n + j];
-        if (edge_less(e.d, e.k, d, k)) { d = e.d; k = e.k; }
-    }
-    best[j].d = d; best[j].k = k;
-}
-
-
-// ------------------------------------------------------------------------------------------------
-// UPGMA on the resident triangle (UPGMA<>::computeTree, UPGMA.cpp:114-295; SURVEY 8f-1).
-//
-// The reference's agglomeration is MUSCLE's nearest-neighbour-cache UPGMA: every live row keeps (MinDist, NearestNeighbor);
-// an iteration picks the live row with the smallest MinDist (first such row), merges it with its cached neighbour,
-// overwrites the row of the left child with the averaged distances and re-labels -- but does not re-evaluate -- the
-// caches of the other rows (UPGMA.cpp:229-262: a row whose neighbour was the right child now points at the left child
-// and keeps the OLD distance).  Results depend on that, so it is reproduced step for step; what is parallel is the inside
-// of a step: both scans (arg-min over the rows, update + arg-min over the new row) are grid-wide reductions of packed
-// (float bits, index) words -- distances are >= 0, so unsigned order is value order and ties go to the lowest index,
-// exactly what the strict < of the sequential scans does.  One cooperative kernel, two grid barriers per merge.
-// ------------------------------------------------------------------------------------------------
-constexpr float kUpgmaBig = 1e29f;                                  // UPGMA::BIG_DIST (UPGMA.h:82)
-constexpr unsigned long long kNoCand = ~0ull;
-
-// Transform<float, Distance> of every pair: the float triangle computeDistances fills (UPGMA.cpp:75-109)
-__global__ void __launch_bounds__(256) k_upgma_dist(const void* __restrict__ tri, int eb, uint32_t n, const uint32_t* __restrict__ lens,
-                                                    const float* __restrict__ pow075, int kind, float never, float* __restrict__ out)
-{
-    const uint32_t i = blockIdx.x + 1;
-    const size_t base = (size_t)i * (i - 1) / 2;
-    const uint32_t li = lens[i];
-    for (uint32_t j = threadIdx.x; j < i; j += blockDim.x) {
-        const uint32_t l = eb == 2 ? static_cast<const uint16_t*>(tri)[base + j] : static_cast<const uint32_t*>(tri)[base + j];
-        out[base + j] = transform_f32(kind, l, li, lens[j], pow075, never);
-    }
-}
-
-__device__ __forceinline__ unsigned long long pack_cand(float d, uint32_t j) { return ((unsigned long long)__float_as_uint(d) << 32) | j; }
-__device__ __forceinline__ unsigned long long block_min_u64(unsigned long long v, unsigned long long* sh)
-{
-    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int o = 16; o; o >>= 1) { const unsigned long long x = __shfl_xor_sync(0xffffffffu, v, o); v = x < v ? x : v; }
-    if (lane == 0) sh[warp] = v;
-    __syncthreads();
-    if (warp == 0) {
-        const uint32_t nw = blockDim.x / 32;
-        v = lane < nw ? sh[lane] : kNoCand;
-        for (int o = 16; o; o >>= 1) { const unsigned long long x = __shfl_xor_sync(0xffffffffu, v, o); v = x < v ? x : v; }
-    }
-    return v;                                                        // valid in warp 0
-}
-
-// initial (MinDist, NearestNeighbor) of every row (UPGMA.cpp:183-203): partners are met in ascending index order and
-// only a strictly smaller distance replaces the cache, so the cache is the arg-min with the lowest partner on ties
-__global__ void __launch_bounds__(256) k_upgma_init(const float* __restrict__ dist, uint32_t n, float* __restrict__ mind, uint32_t* __restrict__ nn,
-                                                    int* __restrict__ node)
-{
-    __shared__ unsigned long long sh[32];
-    const uint32_t r = blockIdx.x;
-    unsigned long long best = kNoCand;
-    const size_t base = (size_t)r * (r ? r - 1 : 0) / 2;
-    for (uint32_t p = threadIdx.x; p < n; p += blockDim.x) {
-        if (p == r) continue;
-        const float d = p < r ? dist[base + p] : dist[(size_t)p * (p - 1) / 2 + r];
-        if (d < kUpgmaBig) { const unsigned long long c = pack_cand(d, p); best = c < best ? c : best; }
-    }
-    best = block_min_u64(best, sh);
-    if (threadIdx.x == 0) {
-        mind[r] = best == kNoCand ? kUpgmaBig : __uint_as_float((unsigned)(best >> 32));
-        nn[r] = best == kNoCand ? 0x7fffffffu : (uint32_t)best;
-        node[r] = (int)r;
-    }
-}
-
-template <bool MODIFIED>
-__global__ void __launch_bounds__(1024) k_upgma(float* __restrict__ dist, uint32_t n, float* __restrict__ mind, uint32_t* __restrict__ nn,
-                                                int* __restrict__ node, unsigned long long* __restrict__ cand, int* __restrict__ out_tree,
-                                                int* __restrict__ status)
-{
-    namespace cg = cooperative_groups;
-    cg::grid_group grid = cg::this_grid();
-    __shared__ unsigned long long sh[32];
-    __shared__ unsigned long long sh_pick;
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t gtid = blockIdx.x * blockDim.x + tid, gthreads = gridDim.x * blockDim.x, nblk = gridDim.x;
-    auto tri_at = [](uint32_t a, uint32_t b) -> size_t { const uint32_t hi = a > b ? a : b, lo = a > b ? b : a; return (size_t)hi * (hi - 1) / 2 + lo; };
-    // every block reduces the nblk published candidates of buffer `buf` for itself: all agree without a second barrier
-    auto gather = [&](uint32_t buf) -> unsigned long long {
-        unsigned long long v = kNoCand;
-        if (warp == 0) {
-            for (uint32_t b = lane; b < nblk; b += 32) { const unsigned long long x = cand[(size_t)buf * nblk + b]; v = x < v ? x : v; }
-            for (int o = 16; o; o >>= 1) { const unsigned long long x = __shfl_xor_sync(0xffffffffu, v, o); v = x < v ? x : v; }
-            if (lane == 0) sh_pick = v;
-        }
-        __syncthreads();
-        return sh_pick;
-    };
-    // what the previous merge changed (row L got a new cache, row R died): every thread knows it from the reductions, so the
-    // scan below does not have to wait for thread 0's writes to become visible -- two grid barriers per merge, not three
-    uint32_t pL = 0xffffffffu, pR = 0xffffffffu;
-    unsigned long long pN = kNoCand;
-    for (uint32_t it = 0; it + 1 < n; ++it) {
-        // ---- the live row with the smallest cached distance (first such row)
-        unsigned long long best = kNoCand;
-        for (uint32_t j = gtid; j < n; j += gthreads) {
-            if (j == pR) continue;
-            float d;
-            if (j == pL) { if (pN == kNoCand) continue; d = __uint_as_float((unsigned)(pN >> 32)); }
-            else { if (node[j] < 0) continue; d = mind[j]; }
-            if (d < kUpgmaBig) { const unsigned long long c = pack_cand(d, j); best = c < best ? c : best; }
-        }
-        best = block_min_u64(best, sh);
-        if (tid == 0) cand[(size_t)0 * nblk + blockIdx.x] = best;
-        grid.sync();
-        const unsigned long long pick = gather(0);
-        if (pick == kNoCand) { if (gtid == 0) *status = 1; return; }     // no finite distance left: the reference would index out of range
-        const uint32_t L = (uint32_t)pick, R = nn[L];
-        // ---- distances to the new node overwrite the row of L; the arg-min of the new row becomes L's cache
-        unsigned long long nbest = kNoCand;
-        for (uint32_t j = gtid; j < n; j += gthreads) {
-            if (j == L || j == R || node[j] < 0) continue;
-            const size_t vL = tri_at(L, j), vR = tri_at(R, j);
-            const float dL = dist[vL], dR = dist[vR];
-            const float nd = MODIFIED ? __fadd_rn(__fmul_rn(0.05f, __fadd_rn(dL, dR)), __fmul_rn(0.9f, dR < dL ? dR : dL))
-                                      : __fmul_rn(__fadd_rn(dL, dR), 0.5f);
-            if (nn[j] == R) nn[j] = L;
-            dist[vL] = nd;
-            if (nd < kUpgmaBig) { const unsigned long long c = pack_cand(nd, j); nbest = c < nbest ? c : nbest; }
-        }
-        nbest = block_min_u64(nbest, sh);
-        if (tid == 0) cand[(size_t)1 * nblk + blockIdx.x] = nbest;
-        grid.sync();
-        const unsigned long long npick = gather(1);
-        if (gtid == 0) {
-            out_tree[2 * it] = node[L];
-            out_tree[2 * it + 1] = node[R];
-            node[L] = (int)(n + it);
-            nn[L] = npick == kNoCand ? 0x7fffffffu : (uint32_t)npick;
-            mind[L] = npick == kNoCand ? kUpgmaBig : __uint_as_float((unsigned)(npick >> 32));
-            node[R] = -1;                                                // (visible to everybody after the next barrier)
-        }
-        pL = L; pR = R; pN = npick;
-    }
+    lcs_store(out, elem_bytes, R.out_base + k, lcs);
 }
 
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
 
-int DevBuf::reserve(size_t bytes)
+// (T) pow(i, 0.75) for every possible indel count, computed by the host libm like the reference's table
+template <class T>
+static int upload_pow075(famsa_ctx* ctx, DevBuf& buf, cudaStream_t st)
 {
-    if (bytes <= cap) return FAMSA_OK;
-    release();
-    size_t want = bytes + bytes / 8 + 256;
-    cudaError_t e = cudaMalloc(&p, want);
-    if (e != cudaSuccess) {
-        p = nullptr;
-        cudaGetLastError();          // callers may recover (famsa_lcs_prim falls back): do not leave the error for a later check
-        set_error(std::string("cudaMalloc(") + std::to_string(want) + ") failed: " + cudaGetErrorString(e));
-        return FAMSA_E_NOMEM;
-    }
-    cap = want;
+    std::vector<T> pw((size_t)2 * ctx->lcs.max_len + 2);
+    for (size_t v = 0; v < pw.size(); ++v) pw[v] = (T)pow((double)v, 0.75);
+    FB_TRY(buf.reserve(sizeof(T) * pw.size()));
+    FB_CUDA(cudaMemcpyAsync(buf.p, pw.data(), sizeof(T) * pw.size(), cudaMemcpyHostToDevice, st));
+    FB_CUDA(cudaStreamSynchronize(st));          // pw goes out of scope
     return FAMSA_OK;
-}
-void DevBuf::release()
-{
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
 }
 
 template <int NL>
@@ -1080,13 +579,7 @@ static int lcs_upload_impl(famsa_ctx* ctx, const int8_t* codes, const uint64_t* 
     FB_CUDA(cudaMemcpyAsync(S.d_raw_len.p, lens, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, st));
     FB_CUDA(cudaMemsetAsync(S.d_codes.p, kNoMatch, units * 16 + 64, st));
 
-    {   // (float) pow(i, 0.75) for every possible indel count, computed by the host libm like the reference's table
-        std::vector<float> pw((size_t)2 * S.max_len + 2);
-        for (size_t v = 0; v < pw.size(); ++v) pw[v] = (float)pow((double)v, 0.75);
-        FB_TRY(S.d_pow075.reserve(sizeof(float) * pw.size()));
-        FB_CUDA(cudaMemcpyAsync(S.d_pow075.p, pw.data(), sizeof(float) * pw.size(), cudaMemcpyHostToDevice, st));
-        FB_CUDA(cudaStreamSynchronize(st));          // pw goes out of scope
-    }
+    FB_TRY(upload_pow075<float>(ctx, S.d_pow075, st));
     k_repack<<<(n + 7) / 8, 256, 0, st>>>(S.d_raw_codes.as<int8_t>(), S.d_raw_off.as<uint64_t>(),
                                           S.d_raw_len.as<uint32_t>(), S.d_perm.as<uint32_t>(),
                                           S.d_code_off.as<uint32_t>(), S.d_codes.as<uint8_t>(), n);
@@ -1184,12 +677,11 @@ static int exact_rows(famsa_ctx* ctx, const std::vector<ExactReq>& reqs, const u
 
 void lcs_row_pieces(uint32_t row_begin, uint32_t row_end, int n_pieces, const double* frac, uint32_t* bounds)
 {
-    auto tri = [](uint64_t r) { return r ? r * (r - 1) / 2 : 0; };
-    const uint64_t pairs = tri(row_end) - tri(row_begin);
+    const uint64_t pairs = tri_index(row_end, 0) - tri_index(row_begin, 0);
     bounds[0] = row_begin;
     for (int b = 1; b < n_pieces; ++b) {
         const double share = frac ? (double)pairs * frac[b] : (double)pairs * b / n_pieces;
-        uint32_t r = (uint32_t)((1.0 + std::sqrt(1.0 + 8.0 * ((double)tri(row_begin) + share))) / 2.0);
+        uint32_t r = (uint32_t)((1.0 + std::sqrt(1.0 + 8.0 * ((double)tri_index(row_begin, 0) + share))) / 2.0);
         r = (r + 16) / 32 * 32;
         bounds[b] = std::min(std::max(r, bounds[b - 1]), row_end);
     }
@@ -1241,7 +733,7 @@ int lcs_triangle(famsa_ctx* ctx, uint32_t row_begin, uint32_t row_end, void* d_o
     P.out = d_out;
     P.elem_bytes = elem_bytes;
     P.rows_mode = 0;
-    P.tri_base = (uint64_t)row_begin * (row_begin ? row_begin - 1 : 0) / 2;
+    P.tri_base = tri_index(row_begin, 0);
     std::vector<uint32_t> special;      // rows the tile kernel may not answer for: dropped-carry and over-long rows
     if (quirk_fixups) std::set_union(S.h_quirky.begin(), S.h_quirky.end(), S.h_long.begin(), S.h_long.end(), std::back_inserter(special));
     else special = S.h_long;         // true LCS everywhere: only the rows the tile kernel cannot reach
@@ -1273,7 +765,7 @@ int lcs_triangle(famsa_ctx* ctx, uint32_t row_begin, uint32_t row_end, void* d_o
         for (uint32_t row : special) {
             if (row < bounds[b] || row >= bounds[b + 1] || row == 0) continue;
             const bool quirky = quirk_fixups && std::binary_search(S.h_quirky.begin(), S.h_quirky.end(), row);
-            reqs.push_back(ExactReq{row, row, quirky ? 0 : 1, (size_t)row * (row - 1) / 2 - (size_t)P.tri_base});
+            reqs.push_back(ExactReq{row, row, quirky ? 0 : 1, tri_index(row, 0) - (size_t)P.tri_base});
         }
         FB_TRY(exact_rows(ctx, reqs, nullptr, d_out, elem_bytes, bst));
         if (block_events) FB_CUDA(cudaEventRecord(block_events[b], bst));
@@ -1357,120 +849,8 @@ int lcs_rows(famsa_ctx* ctx, const uint32_t* h_ref_ids, uint32_t n_ref, const ui
     return FAMSA_OK;
 }
 
-// Parallel MST (see the kernels above) into `edges`; prim_replay then gives Prim's visiting order.  Expects the true-LCS
-// triangle in d_lcs_tri and the pow table in d_pow075_f64.
-static int prim_boruvka(famsa_ctx* ctx, int kind, int eb, std::vector<MstEdge>& edges)
-{
-    LcsState& S = ctx->lcs;
-    cudaStream_t st = ctx->stream;
-    const uint32_t n = S.n;
-    const size_t pairs = (size_t)n * (n - 1) / 2;
-    const uint32_t n_chunks = (n + kMstChunk - 1) / kMstChunk;
-    FB_TRY(S.d_dist_tri.reserve(pairs * sizeof(double)));
-    FB_TRY(S.d_mst_comp.reserve(sizeof(uint32_t) * n));
-    FB_TRY(S.d_mst_best.reserve(sizeof(EdgeMin) * n));
-    FB_TRY(S.d_mst_part.reserve(sizeof(EdgeMin) * (size_t)n_chunks * n));
-    double* d_dtri = S.d_dist_tri.as<double>();
-    uint32_t* d_comp = S.d_mst_comp.as<uint32_t>();
-    EdgeMin* d_best = S.d_mst_best.as<EdgeMin>();
-    EdgeMin* d_part = S.d_mst_part.as<EdgeMin>();
-    k_mst_dist<<<n - 1, 256, 0, st>>>(S.d_lcs_tri.p, eb, n, S.d_raw_len.as<uint32_t>(), S.d_pow075_f64.as<double>(), kind,
-                                      nextafter(DBL_MAX, 0.0), d_dtri);
-    FB_CUDA(cudaGetLastError());
-    ctx->launches++;
-
-    std::vector<uint32_t> parent(n), comp(n);
-    std::iota(parent.begin(), parent.end(), 0u);
-    std::iota(comp.begin(), comp.end(), 0u);
-    auto find = [&](uint32_t x) {
-        while (parent[x] != x) { parent[x] = parent[parent[x]]; x = parent[x]; }
-        return x;
-    };
-    edges.clear();
-    edges.reserve(n - 1);
-    std::vector<EdgeMin> best(n), cbest(n);
-    const double none = kEdgeNone;
-    uint32_t n_comp = n;
-    while (n_comp > 1) {
-        FB_CUDA(cudaMemcpyAsync(d_comp, comp.data(), sizeof(uint32_t) * n, cudaMemcpyHostToDevice, st));
-        k_mst_rows<<<n, 256, 0, st>>>(d_dtri, n, d_comp, d_best);
-        k_mst_cols<<<dim3((n + 31) / 32, n_chunks), 256, 0, st>>>(d_dtri, n, d_comp, d_part);
-        k_mst_combine<<<(n + 255) / 256, 256, 0, st>>>(n, n_chunks, d_part, d_best);
-        FB_CUDA(cudaGetLastError());
-        ctx->launches += 3;
-        FB_CUDA(cudaMemcpyAsync(best.data(), d_best, sizeof(EdgeMin) * n, cudaMemcpyDeviceToHost, st));
-        FB_CUDA(cudaStreamSynchronize(st));
-        // every component's smallest outgoing edge ...
-        for (uint32_t v = 0; v < n; ++v) cbest[v].d = none;
-        for (uint32_t v = 0; v < n; ++v) {
-            if (!(best[v].d < none)) continue;
-            EdgeMin& c = cbest[comp[v]];
-            if (best[v].d < c.d || (best[v].d == c.d && best[v].k < c.k)) c = best[v];
-        }
-        // ... joins two components (the edge order is strict, so no cycle can close)
-        const uint32_t before = n_comp;
-        for (uint32_t c = 0; c < n; ++c) {
-            if (!(cbest[c].d < none)) continue;
-            const unsigned long long packed = ~cbest[c].k;         // uint64_to_id (MSTPrim.h:441-450)
-            const uint32_t a = (uint32_t)(packed >> 32), b = (uint32_t)(packed & 0xffffffffull);
-            const uint32_t ra = find(a), rb = find(b);
-            if (ra == rb) continue;                                 // both sides elected the same edge
-            parent[ra] = rb;
-            edges.push_back(MstEdge{a, b, cbest[c].d});
-            --n_comp;
-        }
-        if (n_comp == before) { set_error("famsa_lcs_prim: no progress in a Boruvka round"); return FAMSA_E_CUDA; }
-        for (uint32_t v = 0; v < n; ++v) comp[v] = find(v);
-    }
-    return FAMSA_OK;
-}
-
-// Prim's visiting order from vertex 0, replayed on the tree (MSTPrim.cpp:366-386 restricted to tree edges)
-int prim_replay(const std::vector<MstEdge>& edges, int32_t* h_from, int32_t* h_to, double* h_dist, int32_t* h_order)
-{
-    const uint32_t n = (uint32_t)edges.size() + 1;
-    std::vector<std::vector<std::tuple<double, unsigned long long, uint32_t>>> adj(n);
-    for (const MstEdge& e : edges) {
-        const unsigned long long lo = std::min(e.a, e.b), hi = std::max(e.a, e.b);
-        const unsigned long long key = ~((lo << 32) + hi);
-        adj[e.a].emplace_back(e.d, key, e.b);
-        adj[e.b].emplace_back(e.d, key, e.a);
-    }
-    using Item = std::tuple<double, unsigned long long, uint32_t>;
-    std::priority_queue<Item, std::vector<Item>, std::greater<Item>> heap;
-    for (uint32_t v = 0; v < n; ++v) h_order[v] = (int32_t)n;
-    h_order[0] = 0;
-    for (const Item& it : adj[0]) heap.push(it);
-    uint32_t step = 0;
-    while (!heap.empty()) {
-        const Item it = heap.top();
-        heap.pop();
-        const uint32_t v = std::get<2>(it);
-        if (h_order[v] != (int32_t)n) continue;
-        const unsigned long long packed = ~std::get<1>(it);
-        h_from[step] = (int32_t)(packed >> 32);
-        h_to[step] = (int32_t)(packed & 0xffffffffull);
-        h_dist[step] = std::get<0>(it);
-        h_order[v] = (int32_t)++step;
-        for (const Item& nx : adj[v])
-            if (h_order[std::get<2>(nx)] == (int32_t)n) heap.push(nx);
-    }
-    if (step != n - 1) { set_error("famsa_lcs_prim: the replay did not reach every sequence"); return FAMSA_E_CUDA; }
-    return FAMSA_OK;
-}
-
-// (double) pow(i, 0.75) for every possible indel count into d_pow075_f64, host libm, like Transform<double,
-// indel075_div_lcs>'s table
-int lcs_pow075_f64(famsa_ctx* ctx, cudaStream_t st)
-{
-    LcsState& S = ctx->lcs;
-    std::vector<double> pw((size_t)2 * S.max_len + 2);
-    for (size_t v = 0; v < pw.size(); ++v) pw[v] = pow((double)v, 0.75);
-    FB_TRY(S.d_pow075_f64.reserve(sizeof(double) * pw.size()));
-    FB_CUDA(cudaMemcpyAsync(S.d_pow075_f64.p, pw.data(), sizeof(double) * pw.size(), cudaMemcpyHostToDevice, st));
-    FB_CUDA(cudaStreamSynchronize(st));          // pw goes out of scope
-    return FAMSA_OK;
-}
+// (double) pow(i, 0.75) for every possible indel count into d_pow075_f64, like Transform<double, indel075_div_lcs>'s table
+int lcs_pow075_f64(famsa_ctx* ctx, cudaStream_t st) { return upload_pow075<double>(ctx, ctx->lcs.d_pow075_f64, st); }
 
 // out[k * n_col + i] = LCS with sequence rows[k] as the row (seq0) against col_ids[i], by the reference recurrence for
 // every pair (k_lcs_exact_batch / k_lcs_exact): orientation-exact whatever the two sequences are
@@ -1495,237 +875,6 @@ int lcs_side_rows(famsa_ctx* ctx, cudaStream_t st)
     FB_CUDA(cudaMemcpyAsync(S.d_side_idx.p, side_idx.data(), sizeof(int) * n, cudaMemcpyHostToDevice, st));
     FB_TRY(S.d_side_rows.reserve(std::max<size_t>((size_t)nq * n, 1) * sizeof(uint32_t)));
     if (nq) FB_TRY(lcs_rows(ctx, S.h_quirky.data(), nq, nullptr, n, S.d_side_rows.p, 4, st));
-    return FAMSA_OK;
-}
-
-// The sequential vertex loop (k_prim) on d_lcs_tri, d_pow075_f64 and, for MSTPrim, the side rows.  Its outputs stay on
-// the device: edge k joins from[k] < to[k] at dist[k] and was added with the (k+1)-th vertex, order[i] = visiting position.
-struct PrimLoopOut {
-    double* dist;
-    int *from, *to, *order;
-};
-
-template <bool kSlink>
-static int prim_loop(famsa_ctx* ctx, int kind, int eb, cudaStream_t st, PrimLoopOut& o)
-{
-    LcsState& S = ctx->lcs;
-    const uint32_t n = S.n;
-    FB_TRY(S.d_tree_state.reserve((sizeof(PrimState) + 1) * (size_t)n + 64));
-    FB_TRY(S.d_tree_out.reserve((sizeof(int) * 3 + sizeof(double)) * (size_t)n + 64));
-    PrimState* d_state = S.d_tree_state.as<PrimState>();
-    unsigned char* d_vis = reinterpret_cast<unsigned char*>(d_state + n);
-    o.dist = S.d_tree_out.as<double>();
-    o.from = reinterpret_cast<int*>(o.dist + n);
-    o.to = o.from + n;
-    o.order = o.to + n;
-    int per_sm = 0;
-    FB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_prim<kSlink>, 1024, 0));
-    const uint32_t nblk = std::max(1u, std::min((uint32_t)(ctx->sm_count * std::max(per_sm, 1)), (n + 1023) / 1024));
-    FB_TRY(S.d_tree_cand.reserve(sizeof(PrimCand) * 2 * nblk));
-    const void* a_tri = S.d_lcs_tri.p; int a_eb = eb; uint32_t a_n = n;
-    const uint32_t* a_len = S.d_raw_len.as<uint32_t>(); const double* a_pow = S.d_pow075_f64.as<double>();
-    int a_kind = kind; double a_never = nextafter(DBL_MAX, 0.0);
-    const int* a_sidx = kSlink ? nullptr : S.d_side_idx.as<int>();
-    const uint32_t* a_side = kSlink ? nullptr : S.d_side_rows.as<uint32_t>();
-    PrimCand* a_cand = S.d_tree_cand.as<PrimCand>();
-    void* args[] = {&a_tri, &a_eb, &a_n, &a_len, &a_pow, &a_kind, &a_never, &a_sidx, &a_side, &d_state, &d_vis,
-                    &a_cand, &o.from, &o.to, &o.dist, &o.order};
-    FB_CUDA(cudaLaunchCooperativeKernel((void*)k_prim<kSlink>, dim3(nblk), dim3(1024), args, 0, st));
-    ctx->launches++;
-    return FAMSA_OK;
-}
-
-int lcs_prim(famsa_ctx* ctx, int kind, int32_t* h_from, int32_t* h_to, double* h_dist, int32_t* h_order,
-             std::vector<MstEdge>& tree)
-{
-    LcsState& S = ctx->lcs;
-    cudaStream_t st = ctx->stream;
-    const uint32_t n = S.n;
-    const int eb = S.elem_bytes();
-    const size_t pairs = (size_t)n * (n - 1) / 2;
-    FB_TRY(S.d_lcs_tri.reserve(std::max<size_t>(pairs, 1) * eb));
-    // the true-LCS triangle (orientation-free) plus the own rows of the flagged sequences
-    FB_TRY(lcs_triangle(ctx, 0, n, S.d_lcs_tri.p, eb, st, nullptr, 1, nullptr, /*quirk_fixups=*/false));
-    FB_TRY(lcs_side_rows(ctx, st));
-    FB_TRY(lcs_pow075_f64(ctx, st));
-    if (S.h_quirky.empty() && n >= 2 && !getenv("FAMSA_PRIM_SEQUENTIAL")) {
-        const int rc = prim_boruvka(ctx, kind, eb, tree);
-        if (rc != FAMSA_E_NOMEM) return rc;                         // no room for the float64 triangle: sequential loop
-        tree.clear();
-        set_error("");                                              // the failed reservation is not this call's outcome
-    }
-    PrimLoopOut o;
-    FB_TRY(prim_loop<false>(ctx, kind, eb, st, o));
-    if (n > 1) {
-        FB_CUDA(cudaMemcpyAsync(h_from, o.from, sizeof(int) * (n - 1), cudaMemcpyDeviceToHost, st));
-        FB_CUDA(cudaMemcpyAsync(h_to, o.to, sizeof(int) * (n - 1), cudaMemcpyDeviceToHost, st));
-        FB_CUDA(cudaMemcpyAsync(h_dist, o.dist, sizeof(double) * (n - 1), cudaMemcpyDeviceToHost, st));
-    }
-    FB_CUDA(cudaMemcpyAsync(h_order, o.order, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
-    FB_CUDA(cudaStreamSynchronize(st));
-    return FAMSA_OK;
-}
-
-// famsa_lcs_slink: SingleLinkage<>::run (SingleLinkage.cpp:30-189) orders distances by (distance, ids_to_uint64
-// descending), the strict order of the MST engines above, so its hierarchy is the unique MST merged in Kruskal order.
-// The triangle is the one SLINK reads (row i = seq0 against j < i, dropped-carry rows exact), so the distances are
-// symmetric and the Boruvka rounds serve whatever the set; the sequential loop runs when their float64 triangle does not
-// fit or FAMSA_PRIM_SEQUENTIAL is set.  `edges` gets the n-1 MST edges in no particular order; slink_labels names them.
-int lcs_slink(famsa_ctx* ctx, int kind, std::vector<MstEdge>& edges)
-{
-    LcsState& S = ctx->lcs;
-    cudaStream_t st = ctx->stream;
-    const uint32_t n = S.n;
-    const int eb = S.elem_bytes();
-    const size_t pairs = (size_t)n * (n - 1) / 2;
-    edges.clear();
-    if (n < 2) return FAMSA_OK;
-    FB_TRY(S.d_lcs_tri.reserve(pairs * eb));
-    FB_TRY(lcs_triangle(ctx, 0, n, S.d_lcs_tri.p, eb, st, nullptr, 1, nullptr, /*quirk_fixups=*/true));
-    FB_TRY(lcs_pow075_f64(ctx, st));
-    if (!getenv("FAMSA_PRIM_SEQUENTIAL")) {
-        const int rc = prim_boruvka(ctx, kind, eb, edges);
-        if (rc != FAMSA_E_NOMEM) return rc;                         // no room for the float64 triangle: sequential loop
-        edges.clear();
-        set_error("");                                              // the failed reservation is not this call's outcome
-    }
-    PrimLoopOut o;
-    FB_TRY(prim_loop<true>(ctx, kind, eb, st, o));
-    std::vector<int> from(n - 1), to(n - 1);
-    std::vector<double> dist(n - 1);
-    FB_CUDA(cudaMemcpyAsync(from.data(), o.from, sizeof(int) * (n - 1), cudaMemcpyDeviceToHost, st));
-    FB_CUDA(cudaMemcpyAsync(to.data(), o.to, sizeof(int) * (n - 1), cudaMemcpyDeviceToHost, st));
-    FB_CUDA(cudaMemcpyAsync(dist.data(), o.dist, sizeof(double) * (n - 1), cudaMemcpyDeviceToHost, st));
-    FB_CUDA(cudaStreamSynchronize(st));
-    edges.reserve(n - 1);
-    for (uint32_t k = 0; k + 1 < n; ++k) edges.push_back(MstEdge{(uint32_t)from[k], (uint32_t)to[k], dist[k]});
-    return FAMSA_OK;
-}
-
-// SLINK's tree from its MST (famsa_b200/mst.py slink_tree is the same in numpy): the edges in (distance, key) order; for
-// the edge joining clusters whose largest members are a < b, emit (node(a), node(b)) as merge k and key the merged
-// cluster, node n + k, by b.  This is what SLINK's stable_sort of lambda and its index relabelling produce (:166-188).
-void slink_labels(std::vector<MstEdge> edges, uint32_t n, int32_t* tree)
-{
-    auto key = [](const MstEdge& e) { return ~(((unsigned long long)std::min(e.a, e.b) << 32) + std::max(e.a, e.b)); };
-    std::sort(edges.begin(), edges.end(), [&](const MstEdge& x, const MstEdge& y) {
-        return x.d < y.d || (x.d == y.d && key(x) < key(y));
-    });
-    std::vector<uint32_t> parent(n), top(n), node(n);
-    std::iota(parent.begin(), parent.end(), 0u);
-    std::iota(top.begin(), top.end(), 0u);
-    std::iota(node.begin(), node.end(), 0u);
-    auto find = [&](uint32_t x) {
-        while (parent[x] != x) { parent[x] = parent[parent[x]]; x = parent[x]; }
-        return x;
-    };
-    for (size_t k = 0; k < edges.size(); ++k) {
-        const uint32_t ra = find(edges[k].a), rb = find(edges[k].b);
-        const uint32_t lo = std::min(top[ra], top[rb]), hi = std::max(top[ra], top[rb]);
-        tree[2 * k] = (int32_t)node[lo];
-        tree[2 * k + 1] = (int32_t)node[hi];
-        node[hi] = n + (uint32_t)k;
-        parent[ra] = rb;
-        top[rb] = hi;
-    }
-}
-
-int lcs_assign(famsa_ctx* ctx, const uint32_t* h_seed_ids, uint32_t n_seeds, int kind, uint32_t* h_assign, float* h_mind)
-{
-    LcsState& S = ctx->lcs;
-    cudaStream_t st = ctx->stream;
-    const uint32_t n = S.n;
-    const int eb = S.elem_bytes();
-    FB_TRY(S.d_assign_lcs.reserve((size_t)eb * n * n_seeds));
-    FB_TRY(S.d_assign.reserve(sizeof(uint32_t) * n));
-    FB_TRY(S.d_mind.reserve(sizeof(float) * n));
-    FB_TRY(S.d_ids_a.reserve(sizeof(uint32_t) * n_seeds));
-    FB_CUDA(cudaMemcpyAsync(S.d_ids_a.p, h_seed_ids, sizeof(uint32_t) * n_seeds, cudaMemcpyHostToDevice, st));
-    // seed k is the row (seq0) of its distance vector, every sequence a column: exactly famsa_lcs_rows
-    FB_TRY(lcs_rows(ctx, h_seed_ids, n_seeds, nullptr, n, S.d_assign_lcs.p, eb, st));
-    const float never = (float)nextafter((double)FLT_MAX, 0.0);
-    k_assign<<<(n + 255) / 256, 256, 0, st>>>(S.d_assign_lcs.p, eb, n, n_seeds, S.d_ids_a.as<uint32_t>(),
-                                             S.d_raw_len.as<uint32_t>(), S.d_pow075.as<float>(), kind, never,
-                                             S.d_assign.as<uint32_t>(), S.d_mind.as<float>());
-    FB_CUDA(cudaGetLastError());
-    ctx->launches++;
-    FB_CUDA(cudaMemcpyAsync(h_assign, S.d_assign.p, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost, st));
-    FB_CUDA(cudaMemcpyAsync(h_mind, S.d_mind.p, sizeof(float) * n, cudaMemcpyDeviceToHost, st));
-    FB_CUDA(cudaStreamSynchronize(st));
-    return FAMSA_OK;
-}
-
-
-// famsa_lcs_upgma: LCS triangle (row = seq0, as calculateDistanceVector builds it) -> float distances -> the agglomeration
-int lcs_upgma(famsa_ctx* ctx, int kind, int modified, int32_t* h_tree, const void* d_tri_in, int tri_eb)
-{
-    LcsState& S = ctx->lcs;
-    cudaStream_t st = ctx->stream;
-    const uint32_t n = S.n;
-    const int eb = d_tri_in ? tri_eb : S.elem_bytes();
-    const size_t pairs = (size_t)n * (n - 1) / 2;
-    const void* d_tri = d_tri_in;
-    if (!d_tri) {
-        FB_TRY(S.d_lcs_tri.reserve(std::max<size_t>(pairs, 1) * eb));
-        FB_TRY(lcs_triangle(ctx, 0, n, S.d_lcs_tri.p, eb, st));
-        d_tri = S.d_lcs_tri.p;
-    }
-    FB_TRY(S.d_dist_tri.reserve(std::max<size_t>(pairs, 1) * sizeof(float)));
-    FB_TRY(S.d_tree_state.reserve((sizeof(float) + sizeof(uint32_t) + sizeof(int)) * (size_t)n + 64));
-    FB_TRY(S.d_tree_out.reserve(sizeof(int) * 2 * (size_t)n + 64));
-    float* d_dist = S.d_dist_tri.as<float>();
-    float* d_mind = S.d_tree_state.as<float>();
-    uint32_t* d_nn = reinterpret_cast<uint32_t*>(d_mind + n);
-    int* d_node = reinterpret_cast<int*>(d_nn + n);
-    int* d_tree = S.d_tree_out.as<int>();
-    int* d_status = d_tree + 2 * (size_t)(n - 1);
-    const float never = (float)nextafter((double)FLT_MAX, 0.0);
-    k_upgma_dist<<<n - 1, 256, 0, st>>>(d_tri, eb, n, S.d_raw_len.as<uint32_t>(), S.d_pow075.as<float>(), kind, never, d_dist);
-    k_upgma_init<<<n, 256, 0, st>>>(d_dist, n, d_mind, d_nn, d_node);
-    FB_CUDA(cudaGetLastError());
-    FB_CUDA(cudaMemsetAsync(d_status, 0, sizeof(int), st));
-    ctx->launches += 2;
-    {
-        void* fn = modified ? (void*)k_upgma<true> : (void*)k_upgma<false>;
-        int per_sm = 0;
-        FB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, 1024, 0));
-        const uint32_t nblk = std::max(1u, std::min((uint32_t)(ctx->sm_count * std::max(per_sm, 1)), (n + 1023) / 1024));
-        FB_TRY(S.d_tree_cand.reserve(sizeof(unsigned long long) * 2 * nblk));
-        uint32_t a_n = n;
-        unsigned long long* a_cand = S.d_tree_cand.as<unsigned long long>();
-        void* args[] = {&d_dist, &a_n, &d_mind, &d_nn, &d_node, &a_cand, &d_tree, &d_status};
-        FB_CUDA(cudaLaunchCooperativeKernel(fn, dim3(nblk), dim3(1024), args, 0, st));
-        ctx->launches++;
-    }
-    int status = 0;
-    FB_CUDA(cudaMemcpyAsync(h_tree, d_tree, sizeof(int) * 2 * (size_t)(n - 1), cudaMemcpyDeviceToHost, st));
-    FB_CUDA(cudaMemcpyAsync(&status, d_status, sizeof(int), cudaMemcpyDeviceToHost, st));
-    FB_CUDA(cudaStreamSynchronize(st));
-    if (status) { set_error("famsa_lcs_upgma: no finite distance left between two clusters (sequences without a common residue)"); return FAMSA_E_INVALID; }
-    return FAMSA_OK;
-}
-
-// famsa_lcs_assign_shard: the seed rows against this shard's slice of the mask groups only, packed for a MIN all-reduce
-int lcs_assign_shard(famsa_ctx* ctx, const uint32_t* h_seed_ids, uint32_t n_seeds, int kind, uint32_t shard, uint32_t n_shards,
-                     long long* d_packed, cudaStream_t st)
-{
-    LcsState& S = ctx->lcs;
-    const uint32_t n = S.n;
-    const int eb = S.elem_bytes();
-    const uint32_t g_begin = (uint32_t)((unsigned long long)S.n_groups * shard / n_shards);
-    const uint32_t g_end = (uint32_t)((unsigned long long)S.n_groups * (shard + 1) / n_shards);
-    FB_TRY(S.d_assign_lcs.reserve((size_t)eb * n * n_seeds));
-    FB_TRY(S.d_ids_a.reserve(sizeof(uint32_t) * n_seeds));
-    FB_CUDA(cudaMemcpyAsync(S.d_ids_a.p, h_seed_ids, sizeof(uint32_t) * n_seeds, cudaMemcpyHostToDevice, st));
-    FB_TRY(lcs_rows(ctx, h_seed_ids, n_seeds, nullptr, n, S.d_assign_lcs.p, eb, st, g_begin, g_end));
-    S.last_pairs = 0;
-    for (uint32_t g = g_begin; g < g_end; ++g) S.last_pairs += (uint64_t)std::min(32u, n - g * 32) * n_seeds;
-    const float never = (float)nextafter((double)FLT_MAX, 0.0);
-    k_assign_packed<<<(n + 255) / 256, 256, 0, st>>>(S.d_assign_lcs.p, eb, n, n_seeds, S.d_ids_a.as<uint32_t>(),
-                                                    S.d_raw_len.as<uint32_t>(), S.d_pow075.as<float>(), kind, never,
-                                                    S.d_invperm.as<uint32_t>(), g_begin, g_end, d_packed);
-    FB_CUDA(cudaGetLastError());
-    ctx->launches++;
     return FAMSA_OK;
 }
 

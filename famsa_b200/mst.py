@@ -62,7 +62,7 @@ def slink_tree(n: int, edges) -> np.ndarray:
     MST merged in Kruskal order, and its relabelling (stable_sort of lambda, then index[pi[j]] = n + k) names a merge
     by the largest member of each side: for the edge joining clusters with largest members a < b, emit
     (node(a), node(b)); the merged cluster becomes node n + k, keyed by b.  edges: n-1 (from, to, dist) in any order.
-    Returns the n-1 merges, (n-1, 2) int32.  famsa_b200/csrc/lcs.cu slink_labels is the same code in C++."""
+    Returns the n-1 merges, (n-1, 2) int32.  famsa_b200/csrc/tree.cu slink_labels is the same code in C++."""
     order = sorted(edges, key=lambda e: (e[2], edge_key(e[0], e[1])))
     parent = list(range(n))
     top = list(range(n))                                # largest member of the cluster rooted here
