@@ -12,7 +12,7 @@ EXPORTED_SYMBOLS = [
     "famsa_abi_version", "famsa_create", "famsa_destroy", "famsa_last_error", "famsa_kernel_launches",
     "famsa_lcs_upload", "famsa_lcs_upload_sorted", "famsa_lcs_sorted_order", "famsa_lcs_last_tiles", "famsa_lcs_n_seqs", "famsa_lcs_triangle", "famsa_lcs_triangle_device",
     "famsa_device_alloc", "famsa_device_free", "famsa_ipc_export", "famsa_ipc_open", "famsa_ipc_close", "famsa_lcs_triangle_exchange",
-    "famsa_lcs_rows", "famsa_lcs_rows_device", "famsa_lcs_assign", "famsa_lcs_assign_shard", "famsa_lcs_upgma", "famsa_lcs_upgma_from_triangle", "famsa_lcs_prim", "famsa_lcs_slink", "famsa_dist_export", "famsa_transform_f64", "famsa_transform_f32",
+    "famsa_lcs_rows", "famsa_lcs_rows_device", "famsa_lcs_assign", "famsa_lcs_assign_shard", "famsa_lcs_upgma", "famsa_lcs_upgma_from_triangle", "famsa_lcs_prim", "famsa_lcs_slink", "famsa_lcs_nj", "famsa_dist_export", "famsa_transform_f64", "famsa_transform_f32",
     "famsa_lcs_last_timing", "famsa_dp_align_batch", "famsa_dp_align_batch_device", "famsa_dp_last_timing",
     "famsa_prof_set_scoring", "famsa_prof_put", "famsa_prof_merge_batch", "famsa_prof_get", "famsa_prof_drop",
     "famsa_prof_last_timing", "famsa_prof_stats", "famsa_prof_align_tree", "famsa_prof_tree_paths",
@@ -95,6 +95,7 @@ def load_library() -> C.CDLL:
     lib.famsa_lcs_rows_device.argtypes = [vp, vp, u32, vp, u32, vp, i32, vp]
     lib.famsa_lcs_prim.argtypes = [vp, i32, vp, vp, vp, vp]
     lib.famsa_lcs_slink.argtypes = [vp, i32, vp]
+    lib.famsa_lcs_nj.argtypes = [vp, i32, vp]
     lib.famsa_lcs_assign.argtypes = [vp, vp, u32, i32, vp, vp]
     lib.famsa_lcs_upgma.argtypes = [vp, i32, i32, vp]
     lib.famsa_lcs_upgma_from_triangle.argtypes = [vp, i32, i32, vp, i32, vp]
@@ -297,6 +298,12 @@ class Engine:
         t = np.zeros((max(self.n - 1, 1), 2), dtype=np.int32)
         self._check(self.lib.famsa_lcs_slink(self.h, kind, _ptr(t)))
         return t[:max(self.n - 1, 0)]
+
+    def nj(self, kind: int = 0) -> np.ndarray:
+        """famsa_lcs_nj: NeighborJoining's guide tree of the uploaded set, (n-1, 2) child ids of the internal nodes."""
+        t = np.zeros((max(self.n - 1, 1), 2), dtype=np.int32)
+        self._check(self.lib.famsa_lcs_nj(self.h, kind, _ptr(t)))
+        return t[:self.n - 1]
 
     def upgma(self, kind: int = 0, modified: bool = False, d_triangle_ptr: int = 0, elem_bytes: int = 2) -> np.ndarray:
         """famsa_lcs_upgma[_from_triangle]: the UPGMA guide tree of the uploaded set, (n-1, 2) child ids of the internal

@@ -549,6 +549,19 @@ int famsa_lcs_upgma(famsa_ctx* ctx, int distance_kind, int modified, int32_t* tr
     });
 }
 
+int famsa_lcs_nj(famsa_ctx* ctx, int distance_kind, int32_t* tree)
+{
+    return entry(ctx, nullptr, &famsa_ctx::lcs_timing, [&]() -> int {
+        FB_TRY(check_set(ctx, 2));
+        if (!tree) { set_error("NULL argument"); return FAMSA_E_INVALID; }
+        if (distance_kind != 0 && distance_kind != 1) { set_error("NeighborJoining is instantiated for distance_kind 0 and 1 only"); return FAMSA_E_INVALID; }
+        return FAMSA_OK;
+    }, [&](cudaStream_t st) -> int {
+        ctx->lcs.last_pairs = tri_index(ctx->lcs.n, 0);
+        return lcs_timed(ctx, st, [&] { return fb::lcs_nj(ctx, distance_kind, tree); });
+    });
+}
+
 int famsa_lcs_upgma_from_triangle(famsa_ctx* ctx, int distance_kind, int modified, const void* d_triangle, int elem_bytes, int32_t* tree)
 {
     return entry(ctx, nullptr, &famsa_ctx::lcs_timing, [&]() -> int {

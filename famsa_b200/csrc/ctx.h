@@ -76,7 +76,8 @@ struct LcsState {
     DevBuf d_raw_codes, d_raw_off, d_raw_len, d_flags, d_pow075, d_pow075_f64, d_assign_lcs;
     // the guide trees and the export
     DevBuf d_lcs_tri;                        // resident LCS triangle (prim, UPGMA, export), elem_bytes() wide
-    DevBuf d_dist_tri;                       // distance triangle: float64 for the Boruvka rounds, float32 for UPGMA
+    DevBuf d_dist_tri;                       // distance triangle: float64 for the Boruvka rounds, float32 for UPGMA and NJ
+    DevBuf d_nj_half;                        // NJ's compaction target: the float triangle of n/2 + 1 rows
     DevBuf d_side_idx, d_side_rows;          // lcs_side_rows: row of a flagged sequence in d_side_rows or -1; its u32 rows
     DevBuf d_tree_state, d_tree_out, d_tree_cand;   // k_prim's or k_upgma's state, outputs and block candidates
     DevBuf d_mst_comp, d_mst_best, d_mst_part;      // Boruvka rounds
@@ -269,6 +270,7 @@ int lcs_exact_block(famsa_ctx* ctx, const std::vector<uint32_t>& rows, const uin
                     int elem_bytes, cudaStream_t st);
 // tree.cu
 int lcs_upgma(famsa_ctx* ctx, int kind, int modified, int32_t* h_tree, const void* d_tri_in = nullptr, int tri_eb = 2);
+int lcs_nj(famsa_ctx* ctx, int kind, int32_t* h_tree);
 int lcs_assign(famsa_ctx* ctx, const uint32_t* h_seed_ids, uint32_t n_seeds, int kind, uint32_t* h_assign,
                float* h_mind);
 int lcs_assign_shard(famsa_ctx* ctx, const uint32_t* h_seed_ids, uint32_t n_seeds, int kind, uint32_t shard, uint32_t n_shards,

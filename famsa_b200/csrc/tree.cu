@@ -52,6 +52,12 @@ __device__ __forceinline__ bool cand_less(const PrimCand& x, const PrimCand& c)
     return x.id >= 0 && (c.id < 0 || x.dist < c.dist || ((x.dist == c.dist) & (x.key < c.key)));
 }
 __device__ __forceinline__ bool cand_less(unsigned long long x, unsigned long long c) { return x < c; }
+struct NjCand {                    // k_nj's pair (q, a, b), a < b: k = (q in unsigned order << 32) | a; k = ~0 = no candidate
+    unsigned long long k;
+    uint32_t b;
+    uint32_t pad;
+};
+__device__ __forceinline__ bool cand_less(const NjCand& x, const NjCand& c) { return x.k < c.k || ((x.k == c.k) & (x.b < c.b)); }
 
 __device__ __forceinline__ EdgeMin shfl_xor(const EdgeMin& c, int o)
 {
@@ -63,6 +69,10 @@ __device__ __forceinline__ PrimCand shfl_xor(const PrimCand& c, int o)
                     __shfl_xor_sync(0xffffffffu, c.id, o), 0};
 }
 __device__ __forceinline__ unsigned long long shfl_xor(unsigned long long c, int o) { return __shfl_xor_sync(0xffffffffu, c, o); }
+__device__ __forceinline__ NjCand shfl_xor(const NjCand& c, int o)
+{
+    return NjCand{__shfl_xor_sync(0xffffffffu, c.k, o), __shfl_xor_sync(0xffffffffu, c.b, o), 0};
+}
 
 template <class C>
 __device__ __forceinline__ C warp_min(C c)
@@ -433,6 +443,224 @@ __global__ void __launch_bounds__(1024) k_upgma(float* __restrict__ dist, uint32
 }
 
 // ------------------------------------------------------------------------------------------------
+// Neighbour joining on the resident triangle (NeighborJoining<>::computeTree, NeighborJoining.cpp:33-118).
+//
+// The reference keeps the live clusters in ascending original order (erase only, the merged cluster keeps its slot), so
+// a slot order that only ever loses dead slots is its position order, and its first-found tie rule is the lexicographic
+// minimum of (q, a, b).  Per merge, one cooperative kernel with two grid barriers:
+//   1. the Q scan over the live pairs (one warp per row, lanes along it) and its arg-min per block;
+//   2. every block reduces the block candidates itself, then row a, the sums s_k and the node table are updated.
+// The new s_a is a chain of dependent float adds in ascending slot order (:104); it runs in one warp (the last of the
+// grid) during the NEXT scan, which leaves row a and column a to that warp: it sums, then scans the pairs of a.
+// When the live rows fall to half of the stored ones the triangle, s and node are compacted, order preserved, into the
+// other of two buffers (the second a quarter of the first), so each scan reads ~the live triangle only.
+// Dead slots have s = NaN: their q is NaN and never wins, so the scan needs no liveness test per element.
+// ------------------------------------------------------------------------------------------------
+constexpr float kFltMax = 3.40282347e+38f;                       // numeric_limits<float>::max(), min_q's start (:59)
+constexpr uint32_t kNjNone = 0xffffffffu;
+
+// q as an unsigned key that orders like the float (negative values included); -0 and +0 are one key, as they are one value
+__device__ __forceinline__ uint32_t nj_qkey(float q)
+{
+    const uint32_t u = __float_as_uint(__fadd_rn(q, 0.f));       // -0 + 0 = +0
+    return (u >> 31) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ NjCand nj_cand(float q, uint32_t a, uint32_t b)
+{
+    return q < kFltMax ? NjCand{((unsigned long long)nj_qkey(q) << 32) | a, b, 0} : NjCand{~0ull, kNjNone, 0};
+}
+// q of the pair at positions a < b (:69): product, then the earlier position's sum, then the later one's, each rounded
+__device__ __forceinline__ float nj_q(float f, float d, float s_lo, float s_hi) { return __fsub_rn(__fsub_rn(__fmul_rn(f, d), s_lo), s_hi); }
+
+// initial sums (:45-55): s_i = 0, then + D(i, j) for j = 0..n-1, j != i, one add at a time.  One thread per row, 32 rows
+// per warp; tiles left of the diagonal are rows of the warp's own rows, staged through shared memory so the loads stay
+// coalesced, tiles right of it are columns of later rows and coalesced as they are.  Also node[i] = i.
+__global__ void __launch_bounds__(128) k_nj_sums(const float* __restrict__ D, uint32_t n, float* __restrict__ s, int* __restrict__ node)
+{
+    __shared__ float tile[4][32][33];
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint32_t i0 = (blockIdx.x * 4 + warp) * 32, i = i0 + lane;
+    if (i0 >= n) return;
+    float acc = 0.f;
+    for (uint32_t j0 = 0; j0 < n; j0 += 32) {
+        if (j0 < i0) {                                           // j < i for every lane
+            for (uint32_t r = 0; r < 32; ++r) tile[warp][r][lane] = i0 + r < n ? D[tri_index(i0 + r, j0 + lane)] : 0.f;
+            __syncwarp();
+            for (uint32_t jj = 0; jj < 32; ++jj) acc = __fadd_rn(acc, tile[warp][lane][jj]);
+            __syncwarp();
+        } else {
+            for (uint32_t j = j0; j < j0 + 32 && j < n; ++j)
+                if (i < n && j != i) acc = __fadd_rn(acc, D[j < i ? tri_index(i, j) : tri_index(j, i)]);
+        }
+    }
+    if (i < n) { s[i] = acc; node[i] = (int)i; }
+}
+
+// The chain of s_a for the slot merged last, then the pairs of a, by one warp: the candidate of those pairs for lane 0.
+// Lanes load 128 slots at a time, one chunk ahead, and every lane adds them in slot order (the same chain in each lane).
+__device__ __forceinline__ NjCand nj_chain(const float* __restrict__ D, float* __restrict__ s, const int* __restrict__ node,
+                                           uint32_t R, uint32_t pa, float f, uint32_t lane)
+{
+    constexpr uint32_t U = 4;
+    auto dist = [&](uint32_t k) { return D[k < pa ? tri_index(pa, k) : tri_index(k, pa)]; };
+    auto load = [&](uint32_t k0, float (&v)[U], unsigned (&live)[U]) {
+#pragma unroll
+        for (uint32_t u = 0; u < U; ++u) {
+            const uint32_t k = k0 + u * 32 + lane;
+            const bool l = k < R && k != pa && node[k] >= 0;
+            v[u] = l ? dist(k) : 0.f;
+            live[u] = __ballot_sync(0xffffffffu, l);
+        }
+    };
+    float sa = 0.f;
+    float v[U], nv[U];
+    unsigned live[U], nlive[U];
+    load(0, v, live);
+    for (uint32_t k0 = 0; k0 < R; k0 += 32 * U) {
+        if (k0 + 32 * U < R) load(k0 + 32 * U, nv, nlive);
+#pragma unroll
+        for (uint32_t u = 0; u < U; ++u)
+#pragma unroll
+            for (uint32_t j = 0; j < 32; ++j) {
+                const float x = __shfl_sync(0xffffffffu, v[u], j);
+                sa = (live[u] >> j & 1) ? __fadd_rn(sa, x) : sa;
+            }
+#pragma unroll
+        for (uint32_t u = 0; u < U; ++u) { v[u] = nv[u]; live[u] = nlive[u]; }
+    }
+    // pairs (k, a) and (a, k) in ascending k per lane, i.e. in lexicographic order: a strict < keeps the first
+    float bq = kFltMax;
+    uint32_t ba = 0, bb = 0;
+    for (uint32_t k = lane; k < R; k += 32) {
+        if (k == pa || node[k] < 0) continue;
+        const float q = k < pa ? nj_q(f, dist(k), s[k], sa) : nj_q(f, dist(k), sa, s[k]);
+        if (q < bq) { bq = q; ba = k < pa ? k : pa; bb = k < pa ? pa : k; }
+    }
+    if (lane == 0) s[pa] = sa;
+    return nj_cand(bq, ba, bb);
+}
+
+// D0: the float triangle of n rows; D1: room for the triangle of n/2 + 1 rows; s/node: two buffers of n each; map: n
+// entries; misc[0]: the new slot of the pending row after a compaction.  out_tree: the n - 1 merges; *status = 1 when an
+// iteration has no candidate (every q NaN or >= FLT_MAX), where the reference would merge cluster 0 with itself.
+__global__ void __launch_bounds__(1024) k_nj(float* __restrict__ D0, float* __restrict__ D1, uint32_t n, float* __restrict__ s0,
+                                             float* __restrict__ s1, int* __restrict__ node0, int* __restrict__ node1,
+                                             uint32_t* __restrict__ map, uint32_t* __restrict__ misc, NjCand* __restrict__ cand,
+                                             int* __restrict__ out_tree, int* __restrict__ status)
+{
+    namespace cg = cooperative_groups;
+    cg::grid_group grid = cg::this_grid();
+    __shared__ NjCand sh[32];
+    __shared__ NjCand sh_pick;
+    __shared__ uint32_t sh_cnt[32];
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t gtid = blockIdx.x * blockDim.x + tid, gthreads = gridDim.x * blockDim.x, nblk = gridDim.x;
+    const uint32_t gw = blockIdx.x * 32 + warp, n_warps = nblk * 32;
+    const bool chain_warp = gw == n_warps - 1;                   // the scan runs on the other n_warps - 1 warps
+    const NjCand none{~0ull, kNjNone, 0};
+    float* D = D0; float* Dn = D1; float* s = s0; float* sn = s1; int* node = node0; int* noden = node1;
+    uint32_t R = n, pa = kNjNone;                                // stored rows; slot whose s_a chain is pending
+    for (uint32_t it = 0; n - it > 2; ++it) {
+        const uint32_t m = n - it;
+        if (2 * m <= R) {
+            // ---- compaction: block 0 ranks the live slots (map: new -> old) and moves s and node; then all copy the rows
+            if (blockIdx.x == 0) {
+                uint32_t base = 0;
+                for (uint32_t k0 = 0; k0 < R; k0 += blockDim.x) {
+                    const uint32_t k = k0 + tid;
+                    const bool l = k < R && node[k] >= 0;
+                    const unsigned bal = __ballot_sync(0xffffffffu, l);
+                    if (lane == 0) sh_cnt[warp] = __popc(bal);
+                    __syncthreads();
+                    uint32_t pre = 0, total = 0;
+                    for (uint32_t w = 0; w < blockDim.x / 32; ++w) { pre += w < warp ? sh_cnt[w] : 0; total += sh_cnt[w]; }
+                    if (l) {
+                        const uint32_t nk = base + pre + __popc(bal & ((1u << lane) - 1));
+                        map[nk] = k; sn[nk] = s[k]; noden[nk] = node[k];
+                        if (k == pa) misc[0] = nk;
+                    }
+                    base += total;
+                    __syncthreads();
+                }
+            }
+            grid.sync();
+            for (uint32_t r = 1 + gw; r < m; r += n_warps) {
+                const float* src = D + tri_index(map[r], 0);
+                float* dst = Dn + tri_index(r, 0);
+                for (uint32_t c = lane; c < r; c += 32) dst[c] = src[map[c]];
+            }
+            grid.sync();
+            { float* t = D; D = Dn; Dn = t; }
+            { float* t = s; s = sn; sn = t; }
+            { int* t = node; node = noden; noden = t; }
+            R = m;
+            if (pa != kNjNone) pa = misc[0];
+        }
+        // ---- Q scan: every live pair but those of the pending slot, whose sum the chain warp computes meanwhile
+        const float f = (float)(m - 2);
+        NjCand best = none;
+        if (chain_warp) {
+            if (pa != kNjNone) best = nj_chain(D, s, node, R, pa, f, lane);
+        } else {
+            // per lane, rows ascending and columns ascending within a row: (q, c) decides, and an equal (q, c) came first
+            float bq = kFltMax;
+            uint32_t bc = 0, bb = 0;
+            for (uint32_t b = 1 + gw; b < R; b += n_warps - 1) {
+                const float sb = s[b];
+                if (b == pa || isnan(sb)) continue;              // dead row, or every q of the row NaN
+                const float* row = D + tri_index(b, 0);
+                for (uint32_t c = lane; c < b; c += 32) {
+                    if (c == pa) continue;
+                    const float q = nj_q(f, row[c], s[c], sb);
+                    if (q < bq || ((q == bq) & (c < bc))) { bq = q; bc = c; bb = b; }
+                }
+            }
+            best = nj_cand(bq, bc, bb);
+        }
+        best = block_min(best, none, sh);
+        if (tid == 0) cand[blockIdx.x] = best;
+        grid.sync();
+        if (warp == 0) {
+            const NjCand v = warp_min_of(cand, nblk, none);
+            if (lane == 0) sh_pick = v;
+        }
+        __syncthreads();
+        const NjCand pick = sh_pick;
+        if (pick.k == ~0ull) { if (gtid == 0) *status = 1; return; }
+        // ---- merge (:79-113): row a gets (D(a,k) + D(b,k) - D(a,b)) / 2, every other live sum loses D(a,k) + D(b,k) and
+        // gains the new distance; b dies
+        const uint32_t a = (uint32_t)pick.k, b = pick.b;
+        const float dab = D[tri_index(b, a)];
+        for (uint32_t k = gtid; k < R; k += gthreads) {
+            if (k == a || k == b || node[k] < 0) continue;
+            const size_t ia = k < a ? tri_index(a, k) : tri_index(k, a), ib = k < b ? tri_index(b, k) : tri_index(k, b);
+            const float t = __fadd_rn(D[ia], D[ib]);
+            const float nd = __fmul_rn(__fsub_rn(t, dab), 0.5f);
+            s[k] = __fadd_rn(__fsub_rn(s[k], t), nd);
+            D[ia] = nd;
+        }
+        if (gtid == 0) {
+            out_tree[2 * it] = node[a];
+            out_tree[2 * it + 1] = node[b];
+            node[a] = (int)(n + it);
+            node[b] = -1;
+            s[b] = __int_as_float(0x7fc00000);                    // NaN: no pair of b is a candidate any more
+        }
+        pa = a;
+        grid.sync();
+    }
+    // the last two clusters, in position order (:117)
+    if (gtid == 0) {
+        int first = -1;
+        for (uint32_t k = 0; k < R; ++k) {
+            if (node[k] < 0) continue;
+            if (first < 0) first = node[k];
+            else { out_tree[2 * (n - 2)] = first; out_tree[2 * (n - 2) + 1] = node[k]; break; }
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
 
@@ -767,6 +995,56 @@ int lcs_upgma(famsa_ctx* ctx, int kind, int modified, int32_t* h_tree, const voi
     FB_CUDA(cudaMemcpyAsync(&status, d_status, sizeof(int), cudaMemcpyDeviceToHost, st));
     FB_CUDA(cudaStreamSynchronize(st));
     if (status) { set_error("famsa_lcs_upgma: no finite distance left between two clusters (sequences without a common residue)"); return FAMSA_E_INVALID; }
+    return FAMSA_OK;
+}
+
+// famsa_lcs_nj: the LCS triangle UPGMA reads -> float distances (calculateDistanceMatrix, NeighborJoining.cpp:14-18) ->
+// the initial sums -> the agglomeration.  Needs n >= 2.
+int lcs_nj(famsa_ctx* ctx, int kind, int32_t* h_tree)
+{
+    LcsState& S = ctx->lcs;
+    cudaStream_t st = ctx->stream;
+    const uint32_t n = S.n;
+    const int eb = S.elem_bytes();
+    FB_TRY(S.d_lcs_tri.reserve(tri_index(n, 0) * eb));
+    FB_TRY(S.d_dist_tri.reserve(tri_index(n, 0) * sizeof(float)));
+    FB_TRY(S.d_nj_half.reserve(tri_index(n / 2 + 1, 0) * sizeof(float)));
+    FB_TRY(S.d_tree_state.reserve((sizeof(float) * 2 + sizeof(int) * 2 + sizeof(uint32_t)) * (size_t)n + 64));
+    FB_TRY(S.d_tree_out.reserve(sizeof(int) * 2 * (size_t)n + 64));
+    float* d_s0 = S.d_tree_state.as<float>();
+    float* d_s1 = d_s0 + n;
+    int* d_node0 = reinterpret_cast<int*>(d_s1 + n);
+    int* d_node1 = d_node0 + n;
+    uint32_t* d_map = reinterpret_cast<uint32_t*>(d_node1 + n);
+    uint32_t* d_misc = d_map + n;
+    int* d_tree = S.d_tree_out.as<int>();
+    int* d_status = d_tree + 2 * (size_t)(n - 1);
+    FB_TRY(lcs_triangle(ctx, 0, n, S.d_lcs_tri.p, eb, st));
+    FB_TRY(dist_triangle<float>(ctx, S.d_lcs_tri.p, eb, kind, S.d_pow075.as<float>(), st));
+    float* d_dist = S.d_dist_tri.as<float>();
+    float* d_half = S.d_nj_half.as<float>();
+    k_nj_sums<<<(n + 127) / 128, 128, 0, st>>>(d_dist, n, d_s0, d_node0);
+    FB_CUDA(cudaGetLastError());
+    FB_CUDA(cudaMemsetAsync(d_status, 0, sizeof(int), st));
+    ctx->launches++;
+    // the scan of the first merges reads the whole triangle: blocks for every 64 rows, all co-resident
+    int per_sm = 0;
+    FB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void*)k_nj, 1024, 0));
+    const uint32_t nblk = std::max(1u, std::min((uint32_t)(ctx->sm_count * std::max(per_sm, 1)), (n + 63) / 64));
+    FB_TRY(S.d_tree_cand.reserve(sizeof(NjCand) * nblk));
+    uint32_t a_n = n;
+    NjCand* a_cand = S.d_tree_cand.as<NjCand>();
+    void* args[] = {&d_dist, &d_half, &a_n, &d_s0, &d_s1, &d_node0, &d_node1, &d_map, &d_misc, &a_cand, &d_tree, &d_status};
+    FB_CUDA(cudaLaunchCooperativeKernel((const void*)k_nj, dim3(nblk), dim3(1024), args, 0, st));
+    ctx->launches++;
+    int status = 0;
+    FB_CUDA(cudaMemcpyAsync(h_tree, d_tree, sizeof(int) * 2 * (size_t)(n - 1), cudaMemcpyDeviceToHost, st));
+    FB_CUDA(cudaMemcpyAsync(&status, d_status, sizeof(int), cudaMemcpyDeviceToHost, st));
+    FB_CUDA(cudaStreamSynchronize(st));
+    if (status) {
+        set_error("famsa_lcs_nj: a step without a candidate pair (every Q is NaN or >= FLT_MAX: sequences without a common residue)");
+        return FAMSA_E_INVALID;
+    }
     return FAMSA_OK;
 }
 

@@ -305,6 +305,18 @@ inline std::vector<std::pair<int, int>> SingleLinkageTree(Context& ctx, Distance
     return out;
 }
 
+// NeighborJoining<distance>::run (NeighborJoining.cpp:10-21) on the device: the n - 1 merges, tree_structure's internal-node part
+inline std::vector<std::pair<int, int>> NeighborJoiningTree(Context& ctx, Distance measure)
+{
+    const uint32_t n = famsa_lcs_n_seqs(ctx.get());
+    if (measure == Distance::pairwise_identity) throw std::runtime_error("famsa_b200: NeighborJoining is instantiated for the two indel distances only");
+    std::vector<int32_t> t(2 * (size_t)std::max<uint32_t>(n, 1));
+    check(famsa_lcs_nj(ctx.get(), measure == Distance::indel075_div_lcs ? 0 : 1, t.data()));
+    std::vector<std::pair<int, int>> out;
+    for (uint32_t k = 0; k + 1 < n; ++k) out.emplace_back(t[2 * k], t[2 * k + 1]);
+    return out;
+}
+
 // DistanceCalculator<distance>::run (DistanceCalculator.cpp:10-122) on the device: the -dist_export CSV of the set of
 // the last famsa_lcs_upload (input order) into `os`, byte for byte.  ids: CSequence::id without the leading '>'.
 // Returns the bytes written; a failing stream stops the export and throws.

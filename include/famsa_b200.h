@@ -203,6 +203,20 @@ int famsa_lcs_upgma_from_triangle(famsa_ctx* ctx, int distance_kind, int modifie
  * instantiations.  famsa_lcs_last_timing: n_pairs = the whole triangle.  HOST pointer. */
 int famsa_lcs_slink(famsa_ctx* ctx, int distance_kind, int32_t* tree);
 
+/* The neighbour-joining guide tree (-gt nj): NeighborJoining<distance>::run (src/tree/NeighborJoining.cpp:10-21) =
+ * calculateDistanceMatrix (the float Transform of the triangle famsa_lcs_upgma reads) + computeTree (:33-118), on the
+ * triangle kept in HBM: only the n-1 merges leave the device.  Every step picks the first pair (a, b), a < b in position
+ * order, with the smallest q = ((m - 2) D(a,b) - s_a) - s_b (:69, each operation rounded on its own; NaN and values
+ * >= FLT_MAX never win), and updates the distances and row sums as :79-113 do.  tree[2k], tree[2k+1] = children of
+ * internal node n_seqs + k, leaves 0..n-1 in caller order, which must be FAMSA's length-descending order
+ * (src/msa.cpp:245-256) for the reference's tree; the result is that tree pair for pair.  distance_kind 0
+ * (indel075_div_lcs) or 1 (indel_div_lcs), the two NeighborJoining instantiations (:124-125); needs at least 2 sequences.
+ * A step without any candidate pair (every q NaN or >= FLT_MAX, e.g. four or more sequences no two of which share a
+ * residue; the reference would then merge cluster 0 with itself) returns FAMSA_E_INVALID and the context stays usable.
+ * FAMSA_E_NOMEM when the LCS triangle, the float triangle and the compaction buffer (1/4 of the float triangle) do not
+ * fit.  famsa_lcs_last_timing: n_pairs = the whole triangle.  HOST pointer. */
+int famsa_lcs_nj(famsa_ctx* ctx, int distance_kind, int32_t* tree);
+
 /* The distance-matrix export (-dist_export [-square_matrix] [-pid]): DistanceCalculator<distance>::run
  * (src/tree/DistanceCalculator.cpp:10-122) with its text formatting, num2str / NumericConversions::Double2PChar
  * (src/utils/conversion.h:52-119), on the device.  Works on the set of the last famsa_lcs_upload, in the caller's
