@@ -184,12 +184,8 @@ struct ProfTicket {
     size_t ring_host_end = (size_t)-1, ring_dev_end = (size_t)-1;    // ring positions to release when the batch is collected
     cudaEvent_t done = nullptr;
     unsigned long long done_seq = 0;   // != 0: completion is published in ProfState::h_done instead of an event
-    uint32_t n = 0;
-    std::vector<uint32_t> merged_ids, merged_gen;
+    std::vector<uint32_t> merged_ids, merged_gen;    // one per merge of the batch
     famsa_dp_result* h_results = nullptr;   // filled by the batch's D2H copy
-    uint8_t* h_paths = nullptr;
-    uint64_t path_bytes = 0;
-    uint64_t cells_bound = 0;
 };
 struct ProfSlab {
     void* p = nullptr;

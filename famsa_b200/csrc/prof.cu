@@ -32,6 +32,7 @@
 #include "ctx.h"
 #include "dp_plan.h"
 #include "prof_dev.cuh"
+#include "tree_plan.h"
 
 namespace fb {
 
@@ -182,7 +183,7 @@ void place(ProfState& P, uint32_t id, int slab, size_t* cursor, uint32_t width, 
     ++P.n_live;
 }
 
-int release_entry(famsa_ctx* ctx, uint32_t id)
+void release_entry(famsa_ctx* ctx, uint32_t id)
 {
     ProfState& P = ctx->prof;
     ProfEntry& e = P.entries[id];
@@ -197,7 +198,6 @@ int release_entry(famsa_ctx* ctx, uint32_t id)
     }
     e.slab = -1;
     P.free_ids.push_back(id);
-    return FAMSA_OK;
 }
 
 int check_id(const ProfState& P, uint32_t id, const char* what)
@@ -269,25 +269,30 @@ static cudaEvent_t take_event(ProfState& P)
     return e;
 }
 
-// Queues one batch of independent merges on the context's stream and returns without waiting: leaves, DP + traceback
-// (dp.cu), merged tables (k_prof_construct), then one copy of the result records and paths into h_results / h_paths
-// (pinned memory makes that copy asynchronous too).  Children may be profiles of batches that are still queued -- their
-// widths are then upper bounds on the host and are resolved on the device.  The merged profiles are sized for w1 + w2.
+// A batch of merges resolved into DP jobs (prof_resolve); the leaves get scratch tables for the duration of the batch.
+struct ProfBatch {
+    std::vector<famsa_dp_job> jobs;
+    std::vector<DpJobExt> ext;
+    std::vector<LeafDesc> leaves;
+    std::vector<std::pair<uint32_t, int>> leaf_slot;                 // (job, side) per leaf, in `leaves` order
+    size_t leaf_bytes = 0;                                          // of the leaves' tables
+    uint64_t path_need = 0;                                         // of the jobs' path slots
+};
+
 // Children of a batch of merges -> DP jobs: resident profiles by their tables (and, while they are still queued, the device
-// slot their width will appear in), leaves by a descriptor for later materialisation.
-static int prof_resolve(famsa_ctx* ctx, const famsa_prof_merge* merges, uint32_t n, std::vector<famsa_dp_job>& jobs, std::vector<DpJobExt>& ext,
-                        std::vector<LeafDesc>& leaves, std::vector<std::pair<uint32_t, int>>& leaf_slot, size_t& leaf_bytes)
+// slot their width will appear in), leaves by a descriptor for later materialisation.  host_mapped: as for prof_launch.
+static int prof_resolve(famsa_ctx* ctx, const famsa_prof_merge* merges, uint32_t n, bool host_mapped, ProfBatch& B)
 {
     ProfState& P = ctx->prof;
     LcsState& L = ctx->lcs;
-    jobs.assign(n, famsa_dp_job{});
-    ext.assign(n, DpJobExt{nullptr, nullptr, nullptr});
+    B.jobs.assign(n, famsa_dp_job{});
+    B.ext.assign(n, DpJobExt{nullptr, nullptr, nullptr});
     std::vector<uint8_t> seen(P.entries.size(), 0);
     for (uint32_t k = 0; k < n; ++k) {
         for (int side = 0; side < 2; ++side) {
             const uint32_t c = side ? merges[k].child2 : merges[k].child1;
-            famsa_dp_profile& p = side ? jobs[k].p2 : jobs[k].p1;
-            const uint32_t*& src = side ? ext[k].w2_src : ext[k].w1_src;
+            famsa_dp_profile& p = side ? B.jobs[k].p2 : B.jobs[k].p1;
+            const uint32_t*& src = side ? B.ext[k].w2_src : B.ext[k].w1_src;
             src = nullptr;
             if (c & FAMSA_PROF_LEAF) {
                 const uint32_t seq = c & ~FAMSA_PROF_LEAF;
@@ -296,9 +301,9 @@ static int prof_resolve(famsa_ctx* ctx, const famsa_prof_merge* merges, uint32_t
                 p.width = L.h_len_sorted[L.h_invperm[seq]];
                 p.card = 1;
                 if (!p.width) { set_error("famsa_prof_merge_batch: leaf " + std::to_string(seq) + " is empty"); return FAMSA_E_INVALID; }
-                leaves.push_back(LeafDesc{seq, nullptr, nullptr});
-                leaf_slot.emplace_back(k, side);
-                leaf_bytes += table_bytes(p.width);
+                B.leaves.push_back(LeafDesc{seq, nullptr, nullptr});
+                B.leaf_slot.emplace_back(k, side);
+                B.leaf_bytes += table_bytes(p.width);
             } else {
                 FB_TRY(check_id(P, c, "famsa_prof_merge_batch"));
                 if (seen[c]) { set_error("famsa_prof_merge_batch: profile " + std::to_string(c) + " is used twice"); return FAMSA_E_INVALID; }
@@ -309,28 +314,28 @@ static int prof_resolve(famsa_ctx* ctx, const famsa_prof_merge* merges, uint32_t
             }
         }
     }
+    for (const famsa_dp_job& j : B.jobs) B.path_need += path_slot(j.p1.width, j.p2.width, host_mapped);
     return FAMSA_OK;
 }
 
 // The merged profiles of a batch: one slab, every table sized for the widest alignment possible (w1 + w2 columns),
 // pending until the batch is collected.  Job k publishes its merged width to d_widths[ids[k]]; con[k] (job job_base + k,
 // tile0 left at 0) builds its tables.
-static int place_merged(famsa_ctx* ctx, const std::vector<famsa_dp_job>& jobs, std::vector<DpJobExt>& ext, uint32_t job_base,
-                        std::vector<uint32_t>& ids, std::vector<uint32_t>& gen, std::vector<ConJobDev>& con)
+static int place_merged(famsa_ctx* ctx, ProfBatch& B, uint32_t job_base, std::vector<uint32_t>& ids, std::vector<uint32_t>& gen, std::vector<ConJobDev>& con)
 {
     ProfState& P = ctx->prof;
     size_t slab_bytes = 0;
-    for (const famsa_dp_job& j : jobs) slab_bytes += table_bytes(j.p1.width + j.p2.width);
+    for (const famsa_dp_job& j : B.jobs) slab_bytes += table_bytes(j.p1.width + j.p2.width);
     int slab;
     FB_TRY(new_slab(ctx, slab_bytes, &slab));
     size_t cur = 0;
-    for (uint32_t k = 0; k < (uint32_t)jobs.size(); ++k) {
+    for (uint32_t k = 0; k < (uint32_t)B.jobs.size(); ++k) {
         const uint32_t id = new_entry(P);
-        place(P, id, slab, &cur, jobs[k].p1.width + jobs[k].p2.width, jobs[k].p1.card + jobs[k].p2.card);
+        place(P, id, slab, &cur, B.jobs[k].p1.width + B.jobs[k].p2.width, B.jobs[k].p1.card + B.jobs[k].p2.card);
         P.entries[id].pending = true;
         ids.push_back(id);
         gen.push_back(P.entries[id].gen);
-        ext[k].w_dst = P.d_widths.as<uint32_t>() + id;
+        B.ext[k].w_dst = P.d_widths.as<uint32_t>() + id;
         con.push_back(ConJobDev{P.entries[id].scores, P.entries[id].counters, job_base + k, 0});
     }
     return FAMSA_OK;
@@ -338,54 +343,41 @@ static int place_merged(famsa_ctx* ctx, const std::vector<famsa_dp_job>& jobs, s
 
 // The leaf tables of a batch, one after the other from `base`: completes each leaf's descriptor and points its job's
 // side at the tables.
-static void place_leaves(unsigned char* base, std::vector<LeafDesc>& leaves, const std::vector<std::pair<uint32_t, int>>& leaf_slot,
-                         std::vector<famsa_dp_job>& jobs)
+static void place_leaves(unsigned char* base, ProfBatch& B)
 {
     size_t cur = 0;
-    for (size_t a = 0; a < leaves.size(); ++a) {
-        famsa_dp_profile& p = leaf_slot[a].second ? jobs[leaf_slot[a].first].p2 : jobs[leaf_slot[a].first].p1;
+    for (size_t a = 0; a < B.leaves.size(); ++a) {
+        famsa_dp_profile& p = B.leaf_slot[a].second ? B.jobs[B.leaf_slot[a].first].p2 : B.jobs[B.leaf_slot[a].first].p1;
         char* t = reinterpret_cast<char*>(base + cur);
-        leaves[a].scores = reinterpret_cast<long long*>(t);
-        leaves[a].counters = reinterpret_cast<int*>(t + ((size_t)p.width + 1) * kRows * sizeof(long long));
-        p.scores = reinterpret_cast<const int64_t*>(leaves[a].scores);
-        p.counters = leaves[a].counters;
+        B.leaves[a].scores = reinterpret_cast<long long*>(t);
+        B.leaves[a].counters = reinterpret_cast<int*>(t + ((size_t)p.width + 1) * kRows * sizeof(long long));
+        p.scores = reinterpret_cast<const int64_t*>(B.leaves[a].scores);
+        p.counters = B.leaves[a].counters;
         cur += table_bytes(p.width);
     }
 }
 
 // the children of a batch are consumed (msa.cpp:406-407)
-static int release_children(famsa_ctx* ctx, const famsa_prof_merge* merges, uint32_t n)
+static void release_children(famsa_ctx* ctx, const famsa_prof_merge* merges, uint32_t n)
 {
     for (uint32_t k = 0; k < n; ++k)
         for (uint32_t c : {merges[k].child1, merges[k].child2})
-            if (!(c & FAMSA_PROF_LEAF)) FB_TRY(release_entry(ctx, c));
-    return FAMSA_OK;
-}
-
-static bool fused_eligible(const std::vector<famsa_dp_job>& jobs)
-{
-    if (jobs.size() > 4096) return false;
-    for (const famsa_dp_job& j : jobs)
-        if (host_rows(j.p1.width, j.p1.card, j.p2.width, j.p2.card) > 512 || std::max(j.p1.width, j.p2.width) > 8192) return false;
-    if (const char* e = getenv("FAMSA_PROF_FUSED")) return atoi(e) != 0;                            // development knob
-    return true;
+            if (!(c & FAMSA_PROF_LEAF)) release_entry(ctx, c);
 }
 
 // Dependency levels of small merges accumulated for ONE launch of k_merge_fused (every merge whole in one block: leaves,
-// prep, fill, traceback, merged tables; a grid barrier between the levels).  add() does the host bookkeeping of a level
-// right away -- merged profiles get their ids and (upper-bound sized) tables, consumed children are released -- so that
-// the next level can name them; flush() places everything and launches.
+// prep, fill, traceback, merged tables; a grid barrier between the levels).  fused_add() does the host bookkeeping of a
+// level right away -- merged profiles get their ids and (upper-bound sized) tables, consumed children are released -- so
+// that the next level can name them; fused_flush() places everything and launches.
 struct FusedAccum {
-    std::vector<famsa_dp_job> jobs;
-    std::vector<DpJobExt> ext;
-    std::vector<LeafDesc> leaves;
-    std::vector<std::pair<uint32_t, int>> leaf_slot;                 // (job, side), job index over the whole accumulation
+    ProfBatch batch;                                                // the levels one after the other
     std::vector<uint32_t> level_start{0};
     std::vector<uint32_t> merged_ids, merged_gen;
     std::vector<ConJobDev> con;
-    size_t leaf_bytes = 0, dev_bytes_est = 0;
+    size_t dev_bytes_est = 0;
     uint32_t max_level = 0;
-    bool empty() const { return jobs.empty(); }
+    bool empty() const { return batch.jobs.empty(); }
+    uint32_t levels() const { return (uint32_t)level_start.size() - 1; }
 };
 
 static size_t fused_dev_estimate(const famsa_dp_job& j)
@@ -394,35 +386,36 @@ static size_t fused_dev_estimate(const famsa_dp_job& j)
            dp_scratch_bytes(j.p1.width, j.p2.width) + skew_elems(j.p1.width, j.p2.width) + 1024;
 }
 
-// may the level (already resolved into `jobs`) join the accumulation?  Checks the rings conservatively.
-static bool fused_fits(famsa_ctx* ctx, const FusedAccum& A, const std::vector<famsa_dp_job>& jobs)
+// may the level (already resolved into B) join the accumulation?  Checks the rings conservatively.
+static bool fused_fits(famsa_ctx* ctx, const FusedAccum& A, const ProfBatch& B)
 {
     ProfState& P = ctx->prof;
     size_t dev = A.dev_bytes_est;
-    for (const famsa_dp_job& j : jobs) dev += fused_dev_estimate(j);
-    const size_t host = (A.jobs.size() + jobs.size()) * (sizeof(DpJobDev) + sizeof(FusedJob)) + (A.level_start.size() + 2) * sizeof(uint32_t) + 1024;
-    return P.d_ring.fits(dev + 4096) && P.h_ring.fits(host);
+    for (const famsa_dp_job& j : B.jobs) dev += fused_dev_estimate(j);
+    const size_t host = (A.batch.jobs.size() + B.jobs.size()) * (sizeof(DpJobDev) + sizeof(FusedJob)) + (A.level_start.size() + 2) * sizeof(uint32_t) + 1024;
+    return fused_joins(A.levels(), A.batch.jobs.size(), B.jobs.size()) && P.d_ring.fits(dev + 4096) && P.h_ring.fits(host);
 }
 
-static int fused_add(famsa_ctx* ctx, FusedAccum& A, const famsa_prof_merge* merges, uint32_t n, std::vector<famsa_dp_job>& jobs, std::vector<DpJobExt>& ext,
-                     std::vector<LeafDesc>& leaves, std::vector<std::pair<uint32_t, int>>& leaf_slot, size_t leaf_bytes)
+static int fused_add(famsa_ctx* ctx, FusedAccum& A, const famsa_prof_merge* merges, ProfBatch& B)
 {
     ProfState& P = ctx->prof;
-    const uint32_t base = (uint32_t)A.jobs.size();
-    FB_TRY(place_merged(ctx, jobs, ext, base, A.merged_ids, A.merged_gen, A.con));
-    for (const famsa_dp_job& j : jobs) A.dev_bytes_est += fused_dev_estimate(j);
-    for (auto& ls : leaf_slot) ls.first += base;
-    A.jobs.insert(A.jobs.end(), jobs.begin(), jobs.end());
-    A.ext.insert(A.ext.end(), ext.begin(), ext.end());
-    A.leaves.insert(A.leaves.end(), leaves.begin(), leaves.end());
-    A.leaf_slot.insert(A.leaf_slot.end(), leaf_slot.begin(), leaf_slot.end());
-    A.leaf_bytes += leaf_bytes;
-    A.level_start.push_back((uint32_t)A.jobs.size());
-    A.max_level = std::max(A.max_level, n);
+    ProfBatch& S = A.batch;
+    const uint32_t base = (uint32_t)S.jobs.size();
+    FB_TRY(place_merged(ctx, B, base, A.merged_ids, A.merged_gen, A.con));
+    for (const famsa_dp_job& j : B.jobs) A.dev_bytes_est += fused_dev_estimate(j);
+    S.jobs.insert(S.jobs.end(), B.jobs.begin(), B.jobs.end());
+    S.ext.insert(S.ext.end(), B.ext.begin(), B.ext.end());
+    S.leaves.insert(S.leaves.end(), B.leaves.begin(), B.leaves.end());
+    for (const auto& ls : B.leaf_slot) S.leaf_slot.emplace_back(base + ls.first, ls.second);   // job index over the whole accumulation
+    S.leaf_bytes += B.leaf_bytes;
+    S.path_need += B.path_need;
+    A.level_start.push_back((uint32_t)S.jobs.size());
+    A.max_level = std::max(A.max_level, (uint32_t)B.jobs.size());
     // The children's storage must not be handed out again before this launch has been queued: inside one launch there is
     // no kernel boundary that would invalidate a stale L1 line
     P.arena.defer = true;
-    return release_children(ctx, merges, n);
+    release_children(ctx, merges, (uint32_t)B.jobs.size());
+    return FAMSA_OK;
 }
 
 static int fused_flush(famsa_ctx* ctx, FusedAccum& A, const int64_t gaps[4], famsa_dp_result* h_results, uint8_t* h_paths, bool host_mapped, ProfTicket* T)
@@ -430,9 +423,9 @@ static int fused_flush(famsa_ctx* ctx, FusedAccum& A, const int64_t gaps[4], fam
     ProfState& P = ctx->prof;
     LcsState& L = ctx->lcs;
     cudaStream_t st = ctx->stream;
-    const uint32_t n = (uint32_t)A.jobs.size(), n_levels = (uint32_t)A.level_start.size() - 1;
+    const uint32_t n = (uint32_t)A.batch.jobs.size(), n_levels = A.levels();
     DpFusedPlan plan;
-    FB_TRY(dp_fused_plan(A.jobs.data(), A.ext.data(), n, host_mapped, nullptr, &plan));
+    FB_TRY(dp_fused_plan(A.batch.jobs.data(), A.batch.ext.data(), n, host_mapped, nullptr, &plan));
     Layout H, D;
     const size_t ho_jobs = H.add(sizeof(DpJobDev) * n);
     const size_t ho_fj = H.add(sizeof(FusedJob) * n);
@@ -440,7 +433,7 @@ static int fused_flush(famsa_ctx* ctx, FusedAccum& A, const int64_t gaps[4], fam
     const size_t o_res = D.add(sizeof(famsa_dp_result) * n);
     const size_t o_meta = D.add(sizeof(DpMeta) * n);
     const size_t o_path = D.add(std::max<uint64_t>(plan.path_bytes, 1));
-    const size_t o_leaf = D.add(A.leaf_bytes);
+    const size_t o_leaf = D.add(A.batch.leaf_bytes);
     const size_t o_scr = D.add(plan.scratch_bytes);
     const size_t o_skew = D.add(plan.skew_bytes);
     const size_t h_off = P.h_ring.alloc(H.end), d_off = P.d_ring.alloc(D.end);
@@ -451,10 +444,10 @@ static int fused_flush(famsa_ctx* ctx, FusedAccum& A, const int64_t gaps[4], fam
     FusedJob* fj = reinterpret_cast<FusedJob*>(hb + ho_fj);
     uint32_t* hl = reinterpret_cast<uint32_t*>(hb + ho_lv);
     famsa_dp_result* d_results = reinterpret_cast<famsa_dp_result*>(db + o_res);
-    place_leaves(db + o_leaf, A.leaves, A.leaf_slot, A.jobs);
-    FB_TRY(dp_fused_plan(A.jobs.data(), A.ext.data(), n, host_mapped, hj, &plan));    // now with the leaves' tables
+    place_leaves(db + o_leaf, A.batch);
+    FB_TRY(dp_fused_plan(A.batch.jobs.data(), A.batch.ext.data(), n, host_mapped, hj, &plan));    // now with the leaves' tables
     for (uint32_t k = 0; k < n; ++k) { fj[k].leaf[0].seq = fj[k].leaf[1].seq = 0xffffffffu; fj[k].con = A.con[k]; }
-    for (size_t a = 0; a < A.leaves.size(); ++a) fj[A.leaf_slot[a].first].leaf[A.leaf_slot[a].second] = A.leaves[a];
+    for (size_t a = 0; a < A.batch.leaves.size(); ++a) fj[A.batch.leaf_slot[a].first].leaf[A.batch.leaf_slot[a].second] = A.batch.leaves[a];
     memcpy(hl, A.level_start.data(), sizeof(uint32_t) * (n_levels + 1));
     FusedParams FP{fj, hl, n_levels, L.d_raw_codes.as<int8_t>(), L.d_raw_off.as<uint64_t>(), L.d_raw_len.as<uint32_t>(), P.d_sm.as<long long>(),
                    0, P.d_block_counter.as<unsigned>(), nullptr, 0};
@@ -475,7 +468,7 @@ static int fused_flush(famsa_ctx* ctx, FusedAccum& A, const int64_t gaps[4], fam
     // storage of the consumed children may be handed out again from here on (everything later is behind this launch)
     P.arena.flush_deferred();
     T->merged_ids = A.merged_ids; T->merged_gen = A.merged_gen;
-    T->n = n; T->h_results = h_results; T->h_paths = h_paths; T->path_bytes = plan.path_bytes; T->cells_bound = plan.cells;
+    T->h_results = h_results;
     T->ring_host_end = P.h_ring.head; T->ring_dev_end = P.d_ring.head;
     A = FusedAccum();
     return FAMSA_OK;
@@ -497,72 +490,64 @@ static int ensure_rings(famsa_ctx* ctx)
     return FAMSA_OK;
 }
 
+// Queues the merges resolved into B on the context's stream and returns without waiting: leaves, DP + traceback (dp.cu),
+// merged tables (k_prof_construct), then one copy of the result records and paths into h_results / h_paths (pinned
+// memory makes that copy asynchronous too).  Children may be profiles of batches that are still queued -- their widths
+// are then upper bounds on the host and are resolved on the device.  The merged profiles are sized for w1 + w2.
 // host_mapped: h_results / h_paths are mapped pinned memory the device may write to directly (and path slots are 16-byte
-// aligned: job k's path at the running sum of align16(w1 + w2))
-static int prof_launch(famsa_ctx* ctx, const famsa_prof_merge* merges, uint32_t n, const int64_t gaps[4],
-                       famsa_dp_result* h_results, uint8_t* h_paths, uint64_t path_cap, bool host_mapped, ProfTicket* T)
+// aligned: job k's path at the running sum of align16(w1 + w2)).  fused: fused_allowed().
+static int prof_launch(famsa_ctx* ctx, const famsa_prof_merge* merges, ProfBatch& B, const int64_t gaps[4], famsa_dp_result* h_results,
+                       uint8_t* h_paths, uint64_t path_cap, bool host_mapped, bool fused, ProfTicket* T)
 {
     ProfState& P = ctx->prof;
+    const uint32_t n = (uint32_t)B.jobs.size();
     LcsState& L = ctx->lcs;
     cudaStream_t st = ctx->stream;
-
-    // resolve the children; leaves get scratch tables for the duration of the batch
-    std::vector<famsa_dp_job> jobs;
-    std::vector<DpJobExt> ext;
-    std::vector<LeafDesc> leaves;
-    std::vector<std::pair<uint32_t, int>> leaf_slot;                 // (job, side) per leaf, in `leaves` order
-    size_t leaf_bytes = 0;
-    FB_TRY(prof_resolve(ctx, merges, n, jobs, ext, leaves, leaf_slot, leaf_bytes));
-    uint64_t path_need = 0, cells = 0;
-    for (const famsa_dp_job& j : jobs) {
-        path_need += path_slot(j.p1.width, j.p2.width, host_mapped);
-        cells += (uint64_t)j.p1.width * j.p2.width;
-    }
-    if (path_need > path_cap) {
-        set_error("famsa_prof_merge_batch: path_buf holds " + std::to_string(path_cap) + " bytes, " + std::to_string(path_need) + " needed");
+    if (B.path_need > path_cap) {
+        set_error("famsa_prof_merge_batch: path_buf holds " + std::to_string(path_cap) + " bytes, " + std::to_string(B.path_need) + " needed");
         return FAMSA_E_INVALID;
     }
     FB_TRY(ensure_widths(ctx, P.entries.size() + n));
     // A batch of small merges only (the chain-like parts of a guide tree: every level one or a few short merges) runs
     // every merge whole in one block of k_merge_fused instead of five launches.
-    if (fused_eligible(jobs)) {
+    if (fused_eligible(fused, B.jobs)) {
         FB_TRY(ensure_rings(ctx));
         FusedAccum A;
-        if (fused_fits(ctx, A, jobs)) {
-            FB_TRY(fused_add(ctx, A, merges, n, jobs, ext, leaves, leaf_slot, leaf_bytes));
+        if (fused_fits(ctx, A, B)) {
+            FB_TRY(fused_add(ctx, A, merges, B));
             return fused_flush(ctx, A, gaps, h_results, h_paths, host_mapped, T);
         }
     }
     std::vector<ConJobDev> con;
-    FB_TRY(place_merged(ctx, jobs, ext, 0, T->merged_ids, T->merged_gen, con));
+    FB_TRY(place_merged(ctx, B, 0, T->merged_ids, T->merged_gen, con));
     uint32_t tiles = 0;
     for (uint32_t k = 0; k < n; ++k) {
         con[k].tile0 = tiles;
-        tiles += (jobs[k].p1.width + jobs[k].p2.width + 1 + kConTile - 1) / kConTile;
+        tiles += (B.jobs[k].p1.width + B.jobs[k].p2.width + 1 + kConTile - 1) / kConTile;
     }
     // batch blob: [results][con jobs][leaf descs][paths][leaf tables]
-    Layout B;
-    const size_t o_res = B.add(sizeof(famsa_dp_result) * n);
-    const size_t o_con = B.add(sizeof(ConJobDev) * n);
-    const size_t o_leafd = B.add(sizeof(LeafDesc) * leaves.size());
-    const size_t o_path = B.add(std::max<uint64_t>(path_need, 1));
-    const size_t o_leaf = B.add(leaf_bytes);
+    Layout Lb;
+    const size_t o_res = Lb.add(sizeof(famsa_dp_result) * n);
+    const size_t o_con = Lb.add(sizeof(ConJobDev) * n);
+    const size_t o_leafd = Lb.add(sizeof(LeafDesc) * B.leaves.size());
+    const size_t o_path = Lb.add(std::max<uint64_t>(B.path_need, 1));
+    const size_t o_leaf = Lb.add(B.leaf_bytes);
     unsigned char* blob = nullptr;
     {
-        cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&blob), B.end, st);
+        cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&blob), Lb.end, st);
         if (e != cudaSuccess) { set_error(std::string("cudaMallocAsync for a merge batch failed: ") + cudaGetErrorString(e)); return FAMSA_E_NOMEM; }
     }
     famsa_dp_result* d_results = reinterpret_cast<famsa_dp_result*>(blob + o_res);
     uint8_t* d_path = blob + o_path;
-    place_leaves(blob + o_leaf, leaves, leaf_slot, jobs);
+    place_leaves(blob + o_leaf, B);
     // one upload: construct jobs and leaf descriptors
     std::vector<unsigned char> pack(o_path - o_con);
     memcpy(pack.data(), con.data(), sizeof(ConJobDev) * n);
-    memcpy(pack.data() + (o_leafd - o_con), leaves.data(), sizeof(LeafDesc) * leaves.size());
+    memcpy(pack.data() + (o_leafd - o_con), B.leaves.data(), sizeof(LeafDesc) * B.leaves.size());
     FB_CUDA(cudaEventRecord(P.ev[0], st));
     FB_CUDA(cudaMemcpyAsync(blob + o_con, pack.data(), pack.size(), cudaMemcpyHostToDevice, st));
-    if (!leaves.empty()) {
-        k_prof_leaf<<<(unsigned)leaves.size(), 256, 0, st>>>(reinterpret_cast<const LeafDesc*>(blob + o_leafd), L.d_raw_codes.as<int8_t>(),
+    if (!B.leaves.empty()) {
+        k_prof_leaf<<<(unsigned)B.leaves.size(), 256, 0, st>>>(reinterpret_cast<const LeafDesc*>(blob + o_leafd), L.d_raw_codes.as<int8_t>(),
                                                              L.d_raw_off.as<uint64_t>(), L.d_raw_len.as<uint32_t>(),
                                                              P.d_sm.as<long long>(), gaps[0], gaps[1], gaps[2], gaps[3]);
         FB_CUDA(cudaGetLastError());
@@ -571,7 +556,7 @@ static int prof_launch(famsa_ctx* ctx, const famsa_prof_merge* merges, uint32_t 
     // DP + traceback on the resident tables (dp.cu)
     DpMeta* d_meta = nullptr;
     void* dp_blob = nullptr;
-    FB_TRY(dp_run_device(ctx, jobs.data(), ext.data(), n, gaps, d_results, d_path, nullptr, &d_meta, &dp_blob, st));
+    FB_TRY(dp_run_device(ctx, B.jobs.data(), B.ext.data(), n, gaps, d_results, d_path, nullptr, &d_meta, &dp_blob, st));
     FB_CUDA(cudaEventRecord(P.ev[1], st));
     k_prof_construct<<<tiles, kConThreads, 0, st>>>(reinterpret_cast<const ConJobDev*>(blob + o_con), n, d_meta, d_results, d_path,
                                                     gaps[0], gaps[1], gaps[2], gaps[3]);
@@ -580,13 +565,13 @@ static int prof_launch(famsa_ctx* ctx, const famsa_prof_merge* merges, uint32_t 
     FB_CUDA(cudaEventRecord(P.ev[2], st));
     P.timing_valid = true;
     FB_CUDA(cudaMemcpyAsync(h_results, d_results, sizeof(famsa_dp_result) * n, cudaMemcpyDeviceToHost, st));
-    if (path_need) FB_CUDA(cudaMemcpyAsync(h_paths, d_path, path_need, cudaMemcpyDeviceToHost, st));
+    if (B.path_need) FB_CUDA(cudaMemcpyAsync(h_paths, d_path, B.path_need, cudaMemcpyDeviceToHost, st));
     FB_CUDA(cudaFreeAsync(dp_blob, st));
     FB_CUDA(cudaFreeAsync(blob, st));
-    FB_TRY(release_children(ctx, merges, n));                        // frees are ordered after the construct kernel
+    release_children(ctx, merges, n);                                // frees are ordered after the construct kernel
     T->done = take_event(P);
     FB_CUDA(cudaEventRecord(T->done, st));
-    T->n = n; T->h_results = h_results; T->h_paths = h_paths; T->path_bytes = path_need; T->cells_bound = cells;
+    T->h_results = h_results;
     return FAMSA_OK;
 }
 
@@ -618,7 +603,7 @@ static int prof_collect(famsa_ctx* ctx, ProfTicket* T)
     if (T->ring_host_end != (size_t)-1) { P.h_ring.release_to(T->ring_host_end); T->ring_host_end = (size_t)-1; }
     if (T->ring_dev_end != (size_t)-1) { P.d_ring.release_to(T->ring_dev_end); T->ring_dev_end = (size_t)-1; }
     int rc = FAMSA_OK;
-    for (uint32_t k = 0; k < T->n; ++k) {
+    for (uint32_t k = 0; k < (uint32_t)T->merged_ids.size(); ++k) {
         ProfEntry& e = P.entries[T->merged_ids[k]];
         const famsa_dp_result& r = T->h_results[k];
         if (e.live && e.pending && e.gen == T->merged_gen[k]) {     // (a later batch may already have consumed it)
@@ -640,22 +625,21 @@ int prof_merge_batch(famsa_ctx* ctx, const famsa_prof_merge* merges, uint32_t n,
     FB_TRY(ensure_pool(ctx));
     P.timing_valid = false;
     if (!n) return FAMSA_OK;
+    ProfBatch B;
+    FB_TRY(prof_resolve(ctx, merges, n, false, B));
     ProfTicket T;
-    FB_TRY(prof_launch(ctx, merges, n, gaps, results, path_buf, path_cap, false, &T));
+    FB_TRY(prof_launch(ctx, merges, B, gaps, results, path_buf, path_cap, false, fused_allowed(), &T));
     const int rc = prof_collect(ctx, &T);
     for (uint32_t k = 0; k < n; ++k) merged_ids[k] = T.merged_ids[k];
     return rc;
 }
 
 // ------------------------------------------------------------------------------------------------
-// The whole progressive alignment (CFAMSA::ComputeAlignment, msa.cpp:360-438) as one call.
-//
-// The reference hands a merge to a worker thread as soon as both children are finished, deepest node first
-// (CProfileQueue, queues.cpp:27-40, 127-187).  Here the unit of submission is "every merge that is ready", and the host
-// does not wait for a batch before it queues the next one: all a parent needs from its children on the host side is an
-// upper bound of their widths (to size buffers); the real widths travel on the device.  Several batches are therefore in
-// flight on the stream while the host collects finished ones in the background to tighten its bounds; it only drains
-// the queue when the bounds of the next batch would inflate its scratch beyond what the real widths would need.
+// The whole progressive alignment (CFAMSA::ComputeAlignment, msa.cpp:360-438) as one call.  The reference hands a merge
+// to a worker thread as soon as both children are finished (CProfileQueue, queues.cpp:27-40, 127-187); here every ready
+// merge is submitted at once, and the host queues the next level before the device has finished the last: a parent
+// needs only an upper bound of its children's widths on the host, the real widths travel on the device (DESIGN.md §4c;
+// when the host waits for the device is decided in tree_plan.h).
 // ------------------------------------------------------------------------------------------------
 static int pinned_reserve(void** p, size_t* cap, size_t bytes)
 {
@@ -668,6 +652,156 @@ static int pinned_reserve(void** p, size_t* cap, size_t bytes)
     return FAMSA_OK;
 }
 
+namespace {
+
+// One famsa_prof_align_tree call: the batches in flight, the profiles the merges made, and the levels of small merges
+// accumulated for one fused launch.  A queued profile's entry holds the bound w1 + w2 as its width until it is collected.
+struct TreeRun {
+    struct InFlight { ProfTicket t; std::vector<uint32_t> merge_ids; uint64_t path_base; };
+    famsa_ctx* ctx; ProfState& P;
+    const int32_t* tree; uint32_t n_leaves; const int64_t* gaps; famsa_dp_result* results;   // prof_align_tree's arguments
+    uint32_t max_exact;                                             // widest profile whose real width is known
+    std::vector<uint32_t> merged;                                   // merge k -> the resident profile of node n_leaves + k
+    const bool fused = fused_allowed(), debug = getenv("FAMSA_DP_DEBUG") != nullptr;   // debug: [tree] lines on stderr
+    std::deque<InFlight> q;
+    uint64_t path_cursor = 0;                                       // next free byte of P.h_tree_paths
+    size_t res_cursor = 0;                                          // next free record of P.h_tree_results
+    FusedAccum acc;
+    std::vector<uint32_t> acc_merges;                               // the merges of `acc`, in its job order
+    famsa_tree_stats st{};
+    std::chrono::steady_clock::duration t_collect{}, t_launch{};     // host time in prof_collect / in launches
+
+    uint32_t handle(uint32_t node) const { return node < n_leaves ? FAMSA_PROF_LEAF | node : merged[node - n_leaves]; }
+    // waits for the oldest batch in flight and takes its results
+    int collect_front()
+    {
+        InFlight& f = q.front();
+        const auto t0 = std::chrono::steady_clock::now();
+        const int rc = prof_collect(ctx, &f.t);
+        t_collect += std::chrono::steady_clock::now() - t0;
+        for (size_t a = 0; a < f.merge_ids.size(); ++a) {
+            famsa_dp_result& r = f.t.h_results[a];
+            r.path_offset += f.path_base;
+            results[f.merge_ids[a]] = r;
+            max_exact = std::max(max_exact, r.path_len);
+            st.cells += (uint64_t)r.rows_width * r.cols_width;
+        }
+        q.pop_front();
+        return rc;
+    }
+    // collects from the front until done() holds or nothing is in flight
+    template <class Done> int drain(Done done)
+    {
+        while (!q.empty() && !done()) FB_TRY(collect_front());
+        return FAMSA_OK;
+    }
+    int drain_to(size_t n) { return drain([&] { return q.size() <= n; }); }
+    // a drain: launches the accumulated levels, then waits for the device until at most `keep` batches are in flight
+    int wait(size_t keep) { FB_TRY(flush()); FB_TRY(drain_to(keep)); ++st.n_drains; return FAMSA_OK; }
+    // collects whatever has finished already (tightens the bounds for free)
+    int collect_finished()
+    {
+        return drain([&] { const ProfTicket& t = q.front().t; return !(t.done_seq ? *P.h_done >= t.done_seq : (!t.done || cudaEventQuery(t.done) == cudaSuccess)); });
+    }
+    // Queues one batch at the cursors, which then advance past its records and path_bytes: the level mg resolved into B,
+    // or the accumulated fused launch when B is null.
+    int submit(const std::vector<uint32_t>& merge_ids, uint64_t path_bytes, const famsa_prof_merge* mg = nullptr, ProfBatch* B = nullptr)
+    {
+        q.push_back(InFlight{ProfTicket(), merge_ids, path_cursor});
+        InFlight& f = q.back();
+        const auto t0 = std::chrono::steady_clock::now();
+        const int rc = B ? prof_launch(ctx, mg, *B, gaps, P.h_tree_results + res_cursor, P.h_tree_paths + path_cursor, P.h_tree_paths_cap - path_cursor, true, fused, &f.t)
+                         : fused_flush(ctx, acc, gaps, P.h_tree_results + res_cursor, P.h_tree_paths + path_cursor, true, &f.t);
+        t_launch += std::chrono::steady_clock::now() - t0;
+        if (rc) { q.pop_back(); return rc; }
+        path_cursor += path_bytes;
+        res_cursor += merge_ids.size();
+        ++st.n_batches;
+        st.max_in_flight = std::max<uint32_t>(st.max_in_flight, (uint32_t)q.size());
+        return FAMSA_OK;
+    }
+    // merge level[a] made resident profile ids[a]
+    void name_merged(const std::vector<uint32_t>& level, const uint32_t* ids)
+    {
+        for (size_t a = 0; a < level.size(); ++a) merged[level[a]] = ids[a];
+        st.peak_resident_bytes = std::max<uint64_t>(st.peak_resident_bytes, P.resident_bytes);
+    }
+    // the widest bound among the level's children that are still queued (0: none is)
+    uint32_t pending_child(const std::vector<uint32_t>& level) const
+    {
+        uint32_t bound = 0;
+        for (uint32_t k : level)
+            for (uint32_t c : {(uint32_t)tree[2 * k], (uint32_t)tree[2 * k + 1]})
+                if (c >= n_leaves && P.entries[handle(c)].pending) bound = std::max(bound, P.entries[handle(c)].width);
+        return bound;
+    }
+    // Launches the accumulated levels behind at most kTreeMaxFusedUncollected - 1 uncollected batches, so that the bounds of
+    // the levels being accumulated (sums over the uncollected part of a chain) do not run away.
+    int flush()
+    {
+        if (acc.empty()) return FAMSA_OK;
+        FB_TRY(drain_to(kTreeMaxFusedUncollected - 1));
+        if (debug) fprintf(stderr, "[tree] fused launch: %u levels, %zu merges\n", acc.levels(), acc.batch.jobs.size());
+        FB_TRY(submit(acc_merges, acc.batch.path_need));
+        acc_merges.clear();
+        return FAMSA_OK;
+    }
+    // Consecutive levels of small merges are accumulated into ONE launch of the fused kernel (a grid barrier between the
+    // levels instead of a kernel boundary): the chain-like stretches of a guide tree are a single merge per level.  Any
+    // other level goes launch by launch.
+    int run_level(size_t lv, const std::vector<uint32_t>& level)
+    {
+        std::vector<famsa_prof_merge> mg(level.size());                 // the level's merges by their children's handles
+        for (size_t a = 0; a < level.size(); ++a) mg[a] = famsa_prof_merge{handle((uint32_t)tree[2 * level[a]]), handle((uint32_t)tree[2 * level[a] + 1])};
+        FB_TRY(collect_finished());
+        if (bound_drifted(pending_child(level), max_exact)) FB_TRY(wait(0));
+        ProfBatch B;
+        FB_TRY(prof_resolve(ctx, mg.data(), (uint32_t)mg.size(), true, B));
+        const bool eligible = fused_eligible(fused, B.jobs), path_room = path_cursor + acc.batch.path_need + B.path_need <= P.h_tree_paths_cap;
+        if (eligible && path_room) {
+            if (!fused_fits(ctx, acc, B)) {
+                FB_TRY(flush());
+                FB_TRY(drain_to(kTreeMaxInFlight - 1));
+                FB_TRY(drain([&] { return fused_fits(ctx, acc, B); }));     // ring space comes back in order
+            }
+            if (fused_fits(ctx, acc, B)) {
+                const size_t first = acc.merged_ids.size();
+                FB_TRY(fused_add(ctx, acc, mg.data(), B));
+                name_merged(level, acc.merged_ids.data() + first);
+                acc_merges.insert(acc_merges.end(), level.begin(), level.end());
+                return FAMSA_OK;
+            }
+        }
+        if (debug) {
+            fprintf(stderr, "[tree] level %zu (%zu merges) not fused: eligible %d, path room %d\n", lv, level.size(), (int)eligible, (int)path_room);
+            fprintf(stderr, "        first job: %u (card %u) x %u (card %u)\n", B.jobs[0].p1.width, B.jobs[0].p1.card, B.jobs[0].p2.width, B.jobs[0].p2.card);
+        }
+        FB_TRY(flush());                                                 // this level goes launch by launch: everything before it first
+        FB_TRY(collect_finished());
+        auto resolve = [&] { B = ProfBatch(); return prof_resolve(ctx, mg.data(), (uint32_t)mg.size(), true, B); };   // with the widths collected since
+        FB_TRY(resolve());
+        uint64_t bound_cells = 0;
+        for (const famsa_dp_job& j : B.jobs) bound_cells += (uint64_t)j.p1.width * j.p2.width;
+        const size_t keep = level_keep(pending_child(level) != 0, bound_cells, path_cursor + B.path_need, P.h_tree_paths_cap, q.size());
+        if (keep != (size_t)-1) {
+            FB_TRY(wait(keep));                                      // (nothing is accumulated here)
+            FB_TRY(resolve());
+            if (path_cursor + B.path_need > P.h_tree_paths_cap) {        // nothing in flight now: the arena may move
+                uint8_t* old = P.h_tree_paths;
+                P.h_tree_paths = nullptr; P.h_tree_paths_cap = 0;
+                FB_TRY(pinned_reserve(reinterpret_cast<void**>(&P.h_tree_paths), &P.h_tree_paths_cap, (path_cursor + B.path_need) * 2));
+                memcpy(P.h_tree_paths, old, path_cursor);
+                cudaFreeHost(old);
+            }
+        }
+        FB_TRY(submit(level, B.path_need, mg.data(), &B));
+        name_merged(level, q.back().t.merged_ids.data());
+        return FAMSA_OK;
+    }
+};
+
+} // namespace
+
 int prof_align_tree(famsa_ctx* ctx, const int32_t* tree, uint32_t n_leaves, const int64_t gaps[4], famsa_dp_result* results,
                     uint32_t* root_id, uint64_t* path_bytes, famsa_tree_stats* stats)
 {
@@ -678,239 +812,39 @@ int prof_align_tree(famsa_ctx* ctx, const int32_t* tree, uint32_t n_leaves, cons
     if (n_leaves != L.n) { set_error("famsa_prof_align_tree: the tree has " + std::to_string(n_leaves) + " leaves, " + std::to_string(L.n) + " sequences are uploaded"); return FAMSA_E_INVALID; }
     if (!P.has_scoring) { set_error("famsa_prof_align_tree: famsa_prof_set_scoring first"); return FAMSA_E_STATE; }
     if (n_leaves < 2) { set_error("famsa_prof_align_tree: fewer than two sequences"); return FAMSA_E_INVALID; }
-    const uint32_t n_merges = n_leaves - 1, n_nodes = 2 * n_leaves - 1;
-    // dependency levels; children must precede parents (tree_structure order)
-    std::vector<uint32_t> depth(n_nodes, 0);
+    const uint32_t n_merges = n_leaves - 1;
     std::vector<std::vector<uint32_t>> levels;
-    std::vector<uint8_t> used(n_nodes, 0);
-    for (uint32_t k = 0; k < n_merges; ++k) {
-        const int32_t a = tree[2 * k], b = tree[2 * k + 1];
-        if (a < 0 || b < 0 || (uint32_t)a >= n_leaves + k || (uint32_t)b >= n_leaves + k || a == b || used[a] || used[b]) {
-            set_error("famsa_prof_align_tree: node " + std::to_string(n_leaves + k) + " has invalid children");
-            return FAMSA_E_INVALID;
-        }
-        used[a] = used[b] = 1;
-        const uint32_t d = std::max(depth[a], depth[b]) + 1;
-        depth[n_leaves + k] = d;
-        if (levels.size() < d) levels.resize(d);
-        levels[d - 1].push_back(k);
-    }
+    const int64_t bad = tree_levels(tree, n_leaves, levels);
+    if (bad >= 0) { set_error("famsa_prof_align_tree: node " + std::to_string(bad) + " has invalid children"); return FAMSA_E_INVALID; }
     FB_TRY(ensure_widths(ctx, P.entries.size() + n_merges + 16));
     FB_TRY(pinned_reserve(reinterpret_cast<void**>(&P.h_tree_results), &P.h_tree_results_cap, sizeof(famsa_dp_result) * n_merges));
-
-    std::vector<uint32_t> handle(n_nodes), width(n_nodes);           // width: layout width (bound until collected)
-    for (uint32_t i = 0; i < n_leaves; ++i) { handle[i] = FAMSA_PROF_LEAF | i; width[i] = L.h_len_sorted[L.h_invperm[i]]; }
-    struct InFlight { ProfTicket t; std::vector<uint32_t> merge_ids; uint64_t path_base; size_t res_base; };
-    std::deque<InFlight> q;
-    uint64_t path_cursor = 0, cells = 0;
-    size_t res_cursor = 0;
-    uint32_t n_batches = 0, max_in_flight = 0, n_drains = 0;
-    uint64_t peak_bytes = 0;
-    constexpr size_t kMaxInFlight = 8;
+    TreeRun R{ctx, P, tree, n_leaves, gaps, results, L.max_len, std::vector<uint32_t>(n_merges)};
+    const uint64_t residues = std::accumulate(L.h_len_sorted.begin(), L.h_len_sorted.end(), uint64_t(0));   // (padded with 0)
     FB_CUDA(cudaEventRecord(P.ev_tree[0], ctx->stream));
-    double t_collect = 0, t_launch = 0;
-    uint32_t max_exact = 0;                                         // widest profile whose real width is known
-    for (uint32_t i = 0; i < n_leaves; ++i) max_exact = std::max(max_exact, width[i]);
-    const bool debug = getenv("FAMSA_DP_DEBUG") != nullptr;       // development aid: [tree] lines on stderr
-    auto now = []() { return std::chrono::steady_clock::now(); };
-    auto collect_front = [&]() -> int {
-        InFlight& f = q.front();
-        const auto t0 = now();
-        const int rc = prof_collect(ctx, &f.t);
-        t_collect += std::chrono::duration<double, std::micro>(now() - t0).count();
-        for (size_t a = 0; a < f.merge_ids.size(); ++a) {
-            const uint32_t k = f.merge_ids[a];
-            famsa_dp_result& r = P.h_tree_results[f.res_base + a];
-            r.path_offset += f.path_base;
-            results[k] = r;
-            width[n_leaves + k] = r.path_len;
-            max_exact = std::max(max_exact, r.path_len);
-            cells += (uint64_t)r.rows_width * r.cols_width;
-        }
-        q.pop_front();
-        return rc;
-    };
-    auto finished = [&](const ProfTicket& t) { return t.done_seq ? *P.h_done >= t.done_seq : (!t.done || cudaEventQuery(t.done) == cudaSuccess); };
-    int rc = FAMSA_OK;
     // paths of all merges: one pinned arena, grown only while nothing is in flight
-    uint64_t arena_need = 0;
-    for (uint32_t i = 0; i < n_leaves; ++i) arena_need += width[i];
-    arena_need = arena_need * 8 + (64u << 20);
-    FB_TRY(pinned_reserve(reinterpret_cast<void**>(&P.h_tree_paths), &P.h_tree_paths_cap, arena_need));
-    // Consecutive levels of small merges are accumulated into ONE launch of the fused kernel (a grid barrier between the
-    // levels instead of a kernel boundary): the chain-like stretches of a guide tree are a single merge per level.
+    FB_TRY(pinned_reserve(reinterpret_cast<void**>(&P.h_tree_paths), &P.h_tree_paths_cap, residues * 8 + (64u << 20)));
     FB_TRY(ensure_rings(ctx));
-    FusedAccum acc;
-    std::vector<uint32_t> acc_merges;
-    uint64_t acc_path_base = 0;
-    size_t acc_res_base = 0;
-    uint32_t acc_levels = 0;
-    constexpr uint32_t kMaxFusedLevels = 32;
-    auto flush_acc = [&]() -> int {
-        if (acc.empty()) return FAMSA_OK;
-        // at most two fused launches uncollected: the widths of everything older become exact, which keeps the upper bounds
-        // of the levels being accumulated (sums over the uncollected part of a chain) from running away
-        while (q.size() >= 2) { const int r = collect_front(); if (r) return r; }
-        q.emplace_back();
-        InFlight& f = q.back();
-        f.merge_ids = acc_merges;
-        f.path_base = acc_path_base;
-        f.res_base = acc_res_base;
-        if (debug) fprintf(stderr, "[tree] fused launch: %u levels, %zu merges\n", acc_levels, acc.jobs.size());
-        const auto t0 = now();
-        const int r = fused_flush(ctx, acc, gaps, P.h_tree_results + acc_res_base, P.h_tree_paths + acc_path_base, true, &f.t);
-        t_launch += std::chrono::duration<double, std::micro>(now() - t0).count();
-        if (r) { q.pop_back(); return r; }
-        acc_merges.clear();
-        acc_levels = 0;
-        ++n_batches;
-        max_in_flight = std::max<uint32_t>(max_in_flight, (uint32_t)q.size());
-        return FAMSA_OK;
-    };
-    for (size_t lv = 0; lv < levels.size() && rc == FAMSA_OK; ++lv) {
-        const std::vector<uint32_t>& level = levels[lv];
-        std::vector<famsa_prof_merge> mg(level.size());             // the level's merges by their children's handles
-        for (size_t a = 0; a < level.size(); ++a) {
-            mg[a].child1 = handle[(uint32_t)tree[2 * level[a]]];
-            mg[a].child2 = handle[(uint32_t)tree[2 * level[a] + 1]];
-        }
-        {
-            // small merges: join the accumulation when the level fits
-            while (!q.empty() && finished(q.front().t) && rc == FAMSA_OK) rc = collect_front();
-            if (rc) break;
-            // A queued child is known by an upper bound only (the sum of its children's bounds), and along a chain the bounds
-            // add up level after level however many older levels have been collected since.  Once a bound has drifted far
-            // from anything real, wait for the device: every width becomes exact again.
-            bool drifted = false;
-            for (uint32_t k : level)
-                for (int side = 0; side < 2; ++side) {
-                    const uint32_t c = (uint32_t)tree[2 * k + side];
-                    if (c >= n_leaves && P.entries[handle[c]].pending && width[c] > 1024 + 2 * max_exact) drifted = true;
-                }
-            if (drifted) {
-                rc = flush_acc();
-                while (!q.empty() && rc == FAMSA_OK) rc = collect_front();
-                if (rc) break;
-                ++n_drains;
-            }
-            std::vector<famsa_dp_job> jobs;
-            std::vector<DpJobExt> ext;
-            std::vector<LeafDesc> leaves;
-            std::vector<std::pair<uint32_t, int>> leaf_slot;
-            size_t leaf_bytes = 0;
-            rc = prof_resolve(ctx, mg.data(), (uint32_t)mg.size(), jobs, ext, leaves, leaf_slot, leaf_bytes);
-            if (rc) break;
-            uint64_t path_need = 0;
-            for (const famsa_dp_job& j : jobs) path_need += path_slot(j.p1.width, j.p2.width, true);
-            if (fused_eligible(jobs) && path_cursor + path_need <= P.h_tree_paths_cap) {
-                if (!(acc_levels < kMaxFusedLevels && acc.jobs.size() + jobs.size() <= 8192 && fused_fits(ctx, acc, jobs))) {
-                    rc = flush_acc();
-                    if (rc) break;
-                    while (q.size() >= kMaxInFlight && rc == FAMSA_OK) rc = collect_front();
-                    while (!fused_fits(ctx, acc, jobs) && !q.empty() && rc == FAMSA_OK) rc = collect_front();   // ring space comes back in order
-                    if (rc) break;
-                }
-                if (fused_fits(ctx, acc, jobs)) {
-                    if (acc.empty()) { acc_path_base = path_cursor; acc_res_base = res_cursor; }
-                    const size_t first = acc.merged_ids.size();
-                    rc = fused_add(ctx, acc, mg.data(), (uint32_t)mg.size(), jobs, ext, leaves, leaf_slot, leaf_bytes);
-                    if (rc) break;
-                    for (size_t a = 0; a < level.size(); ++a) {
-                        const uint32_t k = level[a];
-                        handle[n_leaves + k] = acc.merged_ids[first + a];
-                        width[n_leaves + k] = P.entries[acc.merged_ids[first + a]].width;   // the bound w1 + w2
-                    }
-                    acc_merges.insert(acc_merges.end(), level.begin(), level.end());
-                    path_cursor += path_need;
-                    res_cursor += level.size();
-                    ++acc_levels;
-                    peak_bytes = std::max(peak_bytes, P.resident_bytes);
-                    continue;
-                }
-            }
-            if (debug) fprintf(stderr, "[tree] level %zu (%zu merges) not fused: eligible %d, path room %d\n", lv, level.size(), (int)fused_eligible(jobs), (int)(path_cursor + path_need <= P.h_tree_paths_cap)), fprintf(stderr, "        first job: %u (card %u) x %u (card %u)\n", jobs[0].p1.width, jobs[0].p1.card, jobs[0].p2.width, jobs[0].p2.card);
-            rc = flush_acc();                                         // this level goes launch by launch: everything before it first
-            if (rc) break;
-        }
-        // collect whatever has finished already (tightens the bounds for free)
-        while (!q.empty() && finished(q.front().t) && rc == FAMSA_OK) rc = collect_front();
-        if (rc) break;
-        auto level_cost = [&](uint64_t* bound_cells, uint64_t* path_need) {
-            *bound_cells = *path_need = 0;
-            for (uint32_t k : level) {
-                const uint32_t a = (uint32_t)tree[2 * k], b = (uint32_t)tree[2 * k + 1];
-                *bound_cells += (uint64_t)width[a] * width[b];
-                *path_need += path_slot(width[a], width[b], true);
-            }
-        };
-        uint64_t bound_cells, path_need;
-        level_cost(&bound_cells, &path_need);
-        // Run ahead of the device only while that is cheap: a few batches deep, and not when the bounds of this level
-        // (sums of bounds of uncollected children) would make its direction matrices much larger than they need to be.
-        bool pending_child = false;
-        for (uint32_t k : level)
-            for (int s = 0; s < 2; ++s) {
-                const uint32_t c = (uint32_t)tree[2 * k + s];
-                if (c >= n_leaves && P.entries[handle[c]].pending) pending_child = true;
-            }
-        const bool heavy = bound_cells > (64ull << 20);
-        if ((pending_child && heavy) || q.size() >= kMaxInFlight || path_cursor + path_need > P.h_tree_paths_cap) {
-            const bool all = (pending_child && heavy) || path_cursor + path_need > P.h_tree_paths_cap;
-            while (!q.empty() && rc == FAMSA_OK && (all || q.size() >= kMaxInFlight)) rc = collect_front();
-            if (rc) break;
-            ++n_drains;
-            level_cost(&bound_cells, &path_need);
-            if (path_cursor + path_need > P.h_tree_paths_cap) {      // nothing in flight now: the arena may move
-                uint8_t* old = P.h_tree_paths;
-                P.h_tree_paths = nullptr; P.h_tree_paths_cap = 0;
-                FB_TRY(pinned_reserve(reinterpret_cast<void**>(&P.h_tree_paths), &P.h_tree_paths_cap, (path_cursor + path_need) * 2));
-                memcpy(P.h_tree_paths, old, path_cursor);
-                cudaFreeHost(old);
-            }
-        }
-        q.emplace_back();
-        InFlight& f = q.back();
-        f.merge_ids = level;
-        f.path_base = path_cursor;
-        f.res_base = res_cursor;
-        const auto t0 = now();
-        rc = prof_launch(ctx, mg.data(), (uint32_t)mg.size(), gaps, P.h_tree_results + res_cursor, P.h_tree_paths + path_cursor,
-                         P.h_tree_paths_cap - path_cursor, true, &f.t);
-        t_launch += std::chrono::duration<double, std::micro>(now() - t0).count();
-        if (rc) { q.pop_back(); break; }
-        for (size_t a = 0; a < level.size(); ++a) {
-            const uint32_t k = level[a];
-            handle[n_leaves + k] = f.t.merged_ids[a];
-            width[n_leaves + k] = P.entries[f.t.merged_ids[a]].width;       // the bound w1 + w2
-        }
-        path_cursor += path_need;
-        res_cursor += level.size();
-        ++n_batches;
-        max_in_flight = std::max<uint32_t>(max_in_flight, (uint32_t)q.size());
-        peak_bytes = std::max(peak_bytes, P.resident_bytes);
-    }
-    if (rc == FAMSA_OK) rc = flush_acc();
-    while (!q.empty()) { const int r2 = collect_front(); if (rc == FAMSA_OK) rc = r2; }
+    int rc = FAMSA_OK;
+    for (size_t lv = 0; lv < levels.size() && rc == FAMSA_OK; ++lv) rc = R.run_level(lv, levels[lv]);
+    if (rc == FAMSA_OK) rc = R.flush();
+    while (!R.q.empty()) { const int r2 = R.collect_front(); if (rc == FAMSA_OK) rc = r2; }
     if (rc) return rc;
-    if (debug)
-        fprintf(stderr, "[tree] host time: %.0f us in prof_launch, %.0f us waiting in prof_collect, %.0f us total so far, %u batches\n", t_launch, t_collect,
-                std::chrono::duration<double, std::micro>(now() - t_begin).count(), n_batches);
+    using us = std::chrono::duration<double, std::micro>;
+    if (R.debug)
+        fprintf(stderr, "[tree] host time: %.0f us in prof_launch, %.0f us waiting in prof_collect, %.0f us total so far, %u batches\n",
+                us(R.t_launch).count(), us(R.t_collect).count(), us(std::chrono::steady_clock::now() - t_begin).count(), R.st.n_batches);
     FB_CUDA(cudaEventRecord(P.ev_tree[1], ctx->stream));
     FB_CUDA(cudaEventSynchronize(P.ev_tree[1]));
     float dev_ms = 0.f;
     FB_CUDA(cudaEventElapsedTime(&dev_ms, P.ev_tree[0], P.ev_tree[1]));
-    P.tree_path_bytes = path_cursor;
+    P.tree_path_bytes = R.path_cursor;
     P.tree_merges = n_merges;
-    if (root_id) *root_id = handle[n_nodes - 1];
-    if (path_bytes) *path_bytes = path_cursor;
+    if (root_id) *root_id = R.merged[n_merges - 1];
+    if (path_bytes) *path_bytes = R.path_cursor;
     if (stats) {
-        stats->wall_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
-        stats->device_ms = dev_ms;
-        stats->cells = cells;
-        stats->n_batches = n_batches;
-        stats->n_drains = n_drains;
-        stats->max_in_flight = max_in_flight;
-        stats->peak_resident_bytes = peak_bytes;
+        R.st.wall_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
+        R.st.device_ms = dev_ms;
+        *stats = R.st;
     }
     return FAMSA_OK;
 }
@@ -944,7 +878,7 @@ int prof_drop(famsa_ctx* ctx, const uint32_t* ids, uint32_t n)
     for (uint32_t k = 0; k < n; ++k) FB_TRY(check_id(P, ids[k], "famsa_prof_drop"));
     for (uint32_t k = 0; k < n; ++k) {
         if (!P.entries[ids[k]].live) { set_error("famsa_prof_drop: profile listed twice"); return FAMSA_E_INVALID; }
-        FB_TRY(release_entry(ctx, ids[k]));
+        release_entry(ctx, ids[k]);
     }
     return FAMSA_OK;
 }
