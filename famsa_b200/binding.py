@@ -16,6 +16,7 @@ EXPORTED_SYMBOLS = [
     "famsa_lcs_last_timing", "famsa_dp_align_batch", "famsa_dp_align_batch_device", "famsa_dp_last_timing",
     "famsa_prof_set_scoring", "famsa_prof_put", "famsa_prof_merge_batch", "famsa_prof_get", "famsa_prof_drop",
     "famsa_prof_last_timing", "famsa_prof_stats", "famsa_prof_align_tree", "famsa_prof_tree_paths",
+    "famsa_prof_refine", "famsa_prof_refined_rows",
 ]
 
 PROF_LEAF = 0x80000000            # FAMSA_PROF_LEAF
@@ -45,6 +46,15 @@ class TreeStats(C.Structure):
     _fields_ = [("wall_ms", C.c_double), ("device_ms", C.c_double), ("cells", C.c_uint64), ("n_batches", C.c_uint32),
                 ("n_drains", C.c_uint32), ("max_in_flight", C.c_uint32), ("pad", C.c_uint32),
                 ("peak_resident_bytes", C.c_uint64)]
+
+
+class RefineStats(C.Structure):
+    _fields_ = [("wall_ms", C.c_double), ("device_ms", C.c_double), ("n_tries", C.c_uint32), ("n_realigned", C.c_uint32),
+                ("n_accepted", C.c_uint32), ("n_identical", C.c_uint32), ("cells", C.c_uint64)]
+
+
+REFINE_NO_GAP_OPT = 1        # -dgo
+REFINE_NO_TOTAL_SCORE = 2    # -dsp
 
 
 class FamsaError(RuntimeError):
@@ -116,6 +126,9 @@ def load_library() -> C.CDLL:
     lib.famsa_prof_stats.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
     lib.famsa_prof_align_tree.argtypes = [vp, vp, u32, vp, vp, C.POINTER(u32), C.POINTER(u64), vp]
     lib.famsa_prof_tree_paths.argtypes = [vp, vp, u64]
+    lib.famsa_prof_refine.argtypes = [vp, u32, vp, u32, u32, vp, u32, C.c_int, C.POINTER(u32), C.POINTER(u32),
+                                      C.POINTER(C.c_int64), vp]
+    lib.famsa_prof_refined_rows.argtypes = [vp, vp, u64]
     lib.famsa_dp_align_batch.argtypes = [vp, vp, u32, vp, vp, vp, vp]
     lib.famsa_dp_align_batch_device.argtypes = [vp, vp, u32, vp, vp, vp, vp, vp]
     lib.famsa_dp_last_timing.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(u64)]
@@ -488,6 +501,23 @@ class Engine:
                                                    C.byref(nbytes), C.byref(st)))
         self._check(self.lib.famsa_prof_tree_paths(self.h, _ptr(b["path"]), b["path"].size))
         return root.value, {f: getattr(st, f) for f, _ in TreeStats._fields_ if f != "pad"}
+
+    def refine(self, root_id: int, rows, gaps, n_refinements: int = 100, flags: int = 0):
+        """famsa_prof_refine: RefineAlignment of the resident root (consumed) whose alignment is `rows` (n x width codes,
+        GAP = 30, rows sorted by FASTA id).  Returns (refined rows, width, total score, stats dict, refined profile id);
+        stats also holds `kernel_launches`, the launches of the call."""
+        r = np.ascontiguousarray(rows, dtype=np.uint8)
+        g = np.ascontiguousarray(gaps, dtype=np.int64)
+        rid, w, tot = C.c_uint32(), C.c_uint32(), C.c_int64()
+        st = RefineStats()
+        l0 = self.kernel_launches()
+        self._check(self.lib.famsa_prof_refine(self.h, root_id, _ptr(r), r.shape[0], r.shape[1], _ptr(g), n_refinements, flags,
+                                               C.byref(rid), C.byref(w), C.byref(tot), C.byref(st)))
+        stats = {f: getattr(st, f) for f, _ in RefineStats._fields_}
+        stats["kernel_launches"] = self.kernel_launches() - l0
+        out = np.zeros((r.shape[0], w.value), dtype=np.uint8)
+        self._check(self.lib.famsa_prof_refined_rows(self.h, _ptr(out), out.size))
+        return out, w.value, tot.value, stats, rid.value
 
     def prof_get(self, pid: int, tables: bool = True):
         """(scores, counters, card) of a resident profile, or (width, card) with tables=False."""

@@ -197,6 +197,7 @@ void famsa_destroy(famsa_ctx* ctx)
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
     fb::dist_export_release(ctx);
+    fb::refine_release(ctx);
     fb::prof_release_all(ctx);
     if (ctx->dp.h_pinned) cudaFreeHost(ctx->dp.h_pinned);
     for (auto& ev : ctx->ev)
@@ -702,6 +703,28 @@ int famsa_prof_tree_paths(famsa_ctx* ctx, uint8_t* path_buf, uint64_t path_cap)
     if (!path_buf) { set_error("NULL argument"); return FAMSA_E_INVALID; }
     std::lock_guard<std::mutex> lk(ctx->mu);
     return fb::prof_tree_paths(ctx, path_buf, path_cap);
+}
+
+int famsa_prof_refine(famsa_ctx* ctx, uint32_t root_id, const uint8_t* rows, uint32_t n_rows, uint32_t width,
+                      const int64_t gaps[4], uint32_t n_refinements, int flags, uint32_t* refined_id_out, uint32_t* width_out,
+                      int64_t* total_score_out, famsa_refine_stats* stats)
+{
+    return entry(ctx, nullptr, nullptr, [&]() -> int {
+        if (!rows || !gaps || !refined_id_out || !width_out || !total_score_out) { set_error("NULL argument"); return FAMSA_E_INVALID; }
+        if (flags & ~(FAMSA_REFINE_NO_GAP_OPT | FAMSA_REFINE_NO_TOTAL_SCORE)) { set_error("famsa_prof_refine: unknown flags"); return FAMSA_E_INVALID; }
+        return FAMSA_OK;
+    }, [&](cudaStream_t) {
+        return fb::prof_refine(ctx, root_id, rows, n_rows, width, gaps, n_refinements, flags, refined_id_out, width_out, total_score_out, stats);
+    });
+}
+
+int famsa_prof_refined_rows(famsa_ctx* ctx, uint8_t* rows, uint64_t cap)
+{
+    FB_CHECK_CTX(ctx);
+    if (!rows) { set_error("NULL argument"); return FAMSA_E_INVALID; }
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    FB_CUDA(cudaSetDevice(ctx->device));
+    return fb::prof_refined_rows(ctx, rows, cap);
 }
 
 int famsa_prof_get(famsa_ctx* ctx, uint32_t id, uint32_t* width, uint32_t* card, int64_t* scores, int32_t* counters)

@@ -217,6 +217,17 @@ struct ProfState {
     bool timing_valid = false;
 };
 
+// famsa_prof_refine (refine.cu): the alignment being refined and the candidate of the current try, both column-major
+// (n_rows bytes per column, in id order), and the per-try scratch
+struct RefineState {
+    DevBuf d_cur, d_cand, d_side, d_ends, d_rows, d_cols, d_path, d_acc;
+    void* h_pinned = nullptr;      // per-try results coming back: dest vector, widths, gap counts, score terms
+    size_t h_pinned_cap = 0;
+    uint32_t n = 0, width = 0;     // of the refined alignment (famsa_prof_refined_rows)
+    bool have_rows = false;
+    cudaEvent_t ev[2] = {nullptr, nullptr};   // first and last operation of the call (device_ms)
+};
+
 } // namespace fb
 
 struct famsa_ctx {
@@ -243,6 +254,7 @@ struct famsa_ctx {
     fb::DpState dp;
     fb::CallTiming lcs_timing, dp_timing;               // most recent call of each path (dp: main = the DP kernels)
     fb::ProfState prof;
+    fb::RefineState refine;
 };
 
 namespace fb {
@@ -302,6 +314,8 @@ int prof_set_scoring(famsa_ctx* ctx, const int64_t* sm);
 int prof_put(famsa_ctx* ctx, const famsa_dp_profile* profs, uint32_t n, uint32_t* ids);
 int prof_merge_batch(famsa_ctx* ctx, const famsa_prof_merge* merges, uint32_t n, const int64_t gaps[4], uint32_t* merged_ids,
                      famsa_dp_result* results, uint8_t* path_buf, uint64_t path_cap);
+// entries for n profiles with tables of the given widths (uninitialised), in one slab
+int prof_new(famsa_ctx* ctx, uint32_t n, const uint32_t* widths, const uint32_t* cards, uint32_t* ids);
 int prof_get(famsa_ctx* ctx, uint32_t id, uint32_t* width, uint32_t* card, int64_t* scores, int32_t* counters);
 int prof_drop(famsa_ctx* ctx, const uint32_t* ids, uint32_t n);
 int prof_last_timing(famsa_ctx* ctx, float* total_ms, float* construct_ms);
@@ -309,4 +323,10 @@ int prof_align_tree(famsa_ctx* ctx, const int32_t* tree, uint32_t n_leaves, cons
                     uint32_t* root_id, uint64_t* path_bytes, famsa_tree_stats* stats);
 int prof_tree_paths(famsa_ctx* ctx, uint8_t* path_buf, uint64_t cap);
 void prof_release_all(famsa_ctx* ctx);
+// refine.cu
+int prof_refine(famsa_ctx* ctx, uint32_t root_id, const uint8_t* rows, uint32_t n_rows, uint32_t width, const int64_t gaps[4],
+                uint32_t n_refinements, int flags, uint32_t* refined_id, uint32_t* width_out, int64_t* total_score,
+                famsa_refine_stats* stats);
+int prof_refined_rows(famsa_ctx* ctx, uint8_t* rows, uint64_t cap);
+void refine_release(famsa_ctx* ctx);
 } // namespace fb

@@ -222,29 +222,40 @@ int prof_set_scoring(famsa_ctx* ctx, const int64_t* sm)
     return FAMSA_OK;
 }
 
-int prof_put(famsa_ctx* ctx, const famsa_dp_profile* profs, uint32_t n, uint32_t* ids)
+int prof_new(famsa_ctx* ctx, uint32_t n, const uint32_t* widths, const uint32_t* cards, uint32_t* ids)
 {
     ProfState& P = ctx->prof;
     FB_TRY(ensure_pool(ctx));
     if (!n) return FAMSA_OK;
     size_t bytes = 0;
+    for (uint32_t k = 0; k < n; ++k) bytes += table_bytes(widths[k]);
+    int slab;
+    FB_TRY(new_slab(ctx, bytes, &slab));
+    size_t cur = 0;
+    for (uint32_t k = 0; k < n; ++k) {
+        ids[k] = new_entry(P);
+        place(P, ids[k], slab, &cur, widths[k], cards[k]);
+    }
+    return FAMSA_OK;
+}
+
+int prof_put(famsa_ctx* ctx, const famsa_dp_profile* profs, uint32_t n, uint32_t* ids)
+{
+    ProfState& P = ctx->prof;
+    std::vector<uint32_t> widths(n), cards(n);
     for (uint32_t k = 0; k < n; ++k) {
         if (!profs[k].scores || !profs[k].counters || !profs[k].width || !profs[k].card) {
             set_error("famsa_prof_put: profile " + std::to_string(k) + " is empty");
             return FAMSA_E_INVALID;
         }
-        bytes += table_bytes(profs[k].width);
+        widths[k] = profs[k].width; cards[k] = profs[k].card;
     }
-    int slab;
-    FB_TRY(new_slab(ctx, bytes, &slab));
-    size_t cur = 0;
+    FB_TRY(prof_new(ctx, n, widths.data(), cards.data(), ids));
     for (uint32_t k = 0; k < n; ++k) {
-        const uint32_t id = new_entry(P);
-        place(P, id, slab, &cur, profs[k].width, profs[k].card);
+        const uint32_t id = ids[k];
         const size_t cols = (size_t)profs[k].width + 1;
         FB_CUDA(cudaMemcpyAsync(P.entries[id].scores, profs[k].scores, cols * kRows * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
         FB_CUDA(cudaMemcpyAsync(P.entries[id].counters, profs[k].counters, cols * kRows * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-        ids[k] = id;
     }
     FB_CUDA(cudaStreamSynchronize(ctx->stream));
     return FAMSA_OK;

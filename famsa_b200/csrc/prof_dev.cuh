@@ -13,6 +13,13 @@ constexpr int kGO = 25, kGE = 26, kTE = 27, kTO = 28, kGAP = 30, kNAA = 24;   //
 constexpr int kConThreads = 256, kConTile = 64;
 constexpr size_t kColBytes = kRows * (sizeof(long long) + sizeof(int));        // 384 B per profile column
 
+// The four gap lanes of a profile column's scores: `tot` members times each gap cost (CalculateScores, profile.cpp:171-174
+// for column 0 with tot = card, :212-215 for a column with tot residues); the other lanes get 0.
+__device__ __forceinline__ long long gap_lanes(int lane, long long tot, long long go, long long ge, long long to, long long te)
+{
+    return lane == kGO ? go * tot : lane == kGE ? ge * tot : lane == kTO ? to * tot : lane == kTE ? te * tot : 0;
+}
+
 struct LeafDesc {
     uint32_t seq;
     long long* scores;
@@ -32,7 +39,7 @@ __device__ __forceinline__ void leaf_body(const LeafDesc L, const int8_t* __rest
     const int8_t* s = codes + off[L.seq];
     const int lane = threadIdx.x & 31, warp = (int)(threadIdx.x >> 5) - warp_first, nwarps = (int)(blockDim.x >> 5) - warp_first;
     if (warp < 0) return;
-    const long long gapv = lane == kGO ? go : lane == kGE ? ge : lane == kTE ? te : lane == kTO ? to : 0;
+    const long long gapv = gap_lanes(lane, 1, go, ge, to, te);
     for (uint32_t c = warp; c <= n; c += nwarps) {
         long long sc = gapv;
         int cn = 0;
@@ -188,8 +195,7 @@ __device__ __forceinline__ void construct_tile(const ConJob& J, uint32_t k0, Con
             long long os = 0;
             int oc = 0;
             if (k == 0) {                                               // profile.cpp:998-1001
-                const long long tot = (long long)J.cardr + J.cardc;
-                os = lane == kGO ? go * tot : lane == kGE ? ge * tot : lane == kTO ? to * tot : lane == kTE ? te * tot : 0;
+                os = gap_lanes(lane, (long long)J.cardr + J.cardc, go, ge, to, te);
             } else {
                 const int d = s_dir[t + 1], prev = s_dir[t];
                 const uint32_t i = k - s_nh[t], j = k - s_nv[t];

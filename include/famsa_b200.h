@@ -389,6 +389,40 @@ int famsa_prof_last_timing(famsa_ctx* ctx, float* total_ms, float* construct_ms)
 /* Number of resident profiles and the HBM they occupy. */
 int famsa_prof_stats(famsa_ctx* ctx, uint64_t* n_live, uint64_t* resident_bytes);
 
+/* Refinement of the final alignment: replaces CFAMSA::RefineAlignment (src/msa_refinement.cpp:73-217, called at
+ * src/msa.cpp:615) as it runs with no_threads > 1 (the unbanded Align).  Whether to refine at all (-refine_mode, -rt,
+ * msa_refinement.cpp:79-82) stays with the caller; the clamps of n_refinements (:84-92) are applied here.
+ * root_id: the resident profile famsa_prof_align_tree returned; it is consumed.  rows: the alignment that profile
+ * describes, n_rows x width bytes, row-major, residue codes of src/core/defs.h and GAP = 30 (no GUARD), the rows in the
+ * order the refinement loop uses: sorted by CGappedSequence::id, the FASTA id compared byte-wise (:116).  The caller
+ * sorts, since ids are strings.  gaps = {gap_open, gap_ext, gap_term_open, gap_term_ext} as for the merges.
+ * *refined_id_out: resident id of the final profile (the root's own when no candidate was accepted), for
+ * famsa_prof_get / famsa_prof_drop; *width_out, *total_score_out: its width and CalculateTotalScore (0 with
+ * FAMSA_REFINE_NO_TOTAL_SCORE).  The rows themselves: famsa_prof_refined_rows.  Needs famsa_prof_set_scoring
+ * (FAMSA_E_STATE otherwise); FAMSA_E_INVALID for an unknown root, rows that are not the root's (width, count), fewer
+ * than 2 rows, a row without residues, unknown codes or flags, NULL pointers, and an alignment (also a realignment
+ * during the loop) wider than 51 199 columns; FAMSA_E_NOMEM when an allocation fails.  Errors found before the loop
+ * leave the root resident; once the loop has started, a failing call consumes the root and leaves nothing of its own
+ * resident.  The context stays usable after any error. */
+#define FAMSA_REFINE_NO_GAP_OPT     1   /* -dgo: CParams::enable_gap_optimization = false */
+#define FAMSA_REFINE_NO_TOTAL_SCORE 2   /* -dsp: CParams::enable_total_score_calculation = false */
+
+typedef struct {
+    double wall_ms, device_ms;    /* host wall clock of the call; first to last operation on the stream */
+    uint32_t n_tries;             /* i_ref at loop exit */
+    uint32_t n_realigned;         /* i_succ_ref: distinct splits aligned */
+    uint32_t n_accepted;          /* n_ref_succ */
+    uint32_t n_identical;         /* realignments equal to the current alignment (not scored) */
+    uint64_t cells;               /* sum of DP cells */
+} famsa_refine_stats;
+
+int famsa_prof_refine(famsa_ctx* ctx, uint32_t root_id, const uint8_t* rows, uint32_t n_rows, uint32_t width,
+                      const int64_t gaps[4], uint32_t n_refinements, int flags,
+                      uint32_t* refined_id_out, uint32_t* width_out, int64_t* total_score_out,
+                      famsa_refine_stats* stats /* may be NULL */);
+/* The rows of the most recent famsa_prof_refine: n_rows x width_out bytes, row-major, in the order they were given. */
+int famsa_prof_refined_rows(famsa_ctx* ctx, uint8_t* rows, uint64_t cap);
+
 #ifdef __cplusplus
 }
 #endif
