@@ -225,6 +225,7 @@ struct RefineState {
     size_t h_pinned_cap = 0;
     uint32_t n = 0, width = 0;     // of the refined alignment (famsa_prof_refined_rows)
     bool have_rows = false;
+    bool configured = false;       // k_ref_score_runs' dynamic shared-memory limit raised to kMaxHistBytes
     cudaEvent_t ev[2] = {nullptr, nullptr};   // first and last operation of the call (device_ms)
 };
 

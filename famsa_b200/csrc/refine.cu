@@ -506,7 +506,6 @@ struct Run {
             FB_TRY(launch(k_ref_run_ends, blocks(n, 128), 128, 0, A, n, w, E));
             FB_TRY(launch(k_ref_score_cols, blocks(w, kRT / 32), kRT, 0, counters, w, n, ctx->prof.d_sm.as<long long>(), acc));
             const size_t hist = ((size_t)w + 1) * sizeof(int);
-            if (hist > 48u << 10) FB_CUDA(cudaFuncSetAttribute(k_ref_score_runs, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hist));
             FB_TRY(launch(k_ref_score_runs, w, kRT, hist, (const uint32_t*)E, n, w, acc));
         }
         FB_TRY(launch(k_ref_gapstats, w, kRT, 0, A, n, d_stats));
@@ -575,6 +574,13 @@ static int refine_run(famsa_ctx* ctx, uint32_t root_id, const uint8_t* rows, uin
 
     cudaStream_t st = ctx->stream;
     R.have_rows = false;
+    // k_ref_score_runs' limit once per context, before its first launch: without it the default budget is 48 KiB less
+    // the kernel's 384 bytes of static shared memory, which fails widths of 12 192 .. 12 287 columns (and hid the
+    // failure whenever a wider call had raised the limit before)
+    if (!R.configured) {
+        FB_CUDA(cudaFuncSetAttribute(k_ref_score_runs, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxHistBytes));
+        R.configured = true;
+    }
     FB_TRY(R.d_cur.reserve((size_t)n * width));
     FB_TRY(R.d_rows.reserve((size_t)n * 24 + 1024));
     FB_TRY(R.d_acc.reserve(64));

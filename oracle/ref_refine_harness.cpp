@@ -56,11 +56,11 @@ void render(const CGappedSequence* gs, char* out)
     out[at] = 0;
 }
 
-CProfile* from_rows(Session* s, const char* const* rows, uint32_t n)
+CProfile* from_rows(Session* s, const char* const* rows, uint32_t n, const char* const* ids = nullptr)
 {
     auto* p = new CProfile(&s->params, s->atp.get());
     for (uint32_t i = 0; i < n; ++i) {
-        CGappedSequence gs("s" + std::to_string(i), std::string(rows[i]), (int)i, nullptr);
+        CGappedSequence gs(ids ? std::string(ids[i]) : "s" + std::to_string(i), std::string(rows[i]), (int)i, nullptr);
         p->AppendRawSequence(gs);
     }
     // AppendRawSequence takes width = gapped_size - 1 for a row that starts with GUARD (profile.cpp:334-337), one short
@@ -102,6 +102,84 @@ size_t refine_column(std::mt19937& rnd, CProfile* p, std::vector<size_t>& dest, 
     for (size_t j = 0; j < card; ++j)
         dest.emplace_back(p->data[j]->GetSymbol(col_id) == GAP ? first_prof_id : second_prof_id);
     return col_id;
+}
+
+// RefineAlignment (msa_refinement.cpp:77, 84-92, 113-209) on profile_to_refine, which it consumes: the refined rows by
+// sequence number into `refined`, the refined width, totals = {prev_total_score of :114, final total_score}, counts =
+// {i_ref, i_succ_ref, n_ref_succ, identical}; trace: per try {i_ref, column (0: RefineRandom), FNV-1a of the split,
+// identical, accepted, total}, at most max_trace tries; scores / counters: the final CProfile's tables ((width+1) x 32).
+// Rows and tables are written only when the refined width is below stride.
+void refine_loop(Session* s, CProfile* profile_to_refine, uint32_t n_refinements, char* refined, uint32_t stride, uint32_t* width,
+                 int64_t* totals, uint32_t* counts, int64_t* trace, uint32_t max_trace, int64_t* scores, int32_t* counters)
+{
+    CParams* params = &s->params;
+    // msa_refinement.cpp:77, 84-92
+    std::mt19937 rnd_rfn;
+    rnd_rfn.seed(5489u);
+    size_t n_ref = n_refinements;
+    size_t n_seq = profile_to_refine->Size();
+    std::vector<size_t> gap_stats;
+    if (n_ref > 2 * n_seq) n_ref = 2 * n_seq;
+    if (n_ref > 0 && n_ref < 100 && n_seq < 100) n_ref = 100;
+    // :113-209
+    int n_ref_succ = 0, identical = 0;
+    score_t prev_total_score = profile_to_refine->CalculateTotalScore();
+    totals[0] = prev_total_score;
+    std::sort(profile_to_refine->data.begin(), profile_to_refine->data.end(), [](CGappedSequence* p, CGappedSequence* q) { return p->id < q->id; });
+    std::vector<size_t> dest_prof_id;
+    std::vector<std::vector<size_t>> old_dest_prof_ids;
+    std::vector<int> column_mapping1, column_mapping2;
+    size_t i_ref, i_succ_ref;
+    bool valid_gap_stats = false;
+    for (i_ref = i_succ_ref = 0; i_succ_ref < n_ref && i_ref < 20 * n_ref; ++i_ref) {
+        CProfile profile1(params, s->atp.get()), profile2(params, s->atp.get());
+        const size_t col = refine_column(rnd_rfn, profile_to_refine, dest_prof_id, gap_stats, valid_gap_stats);
+        valid_gap_stats = true;
+        uint32_t hash = 2166136261u;
+        for (size_t d : dest_prof_id) hash = (hash ^ (uint32_t)d) * 16777619u;
+        int64_t* tr = i_ref < max_trace ? trace + 6 * i_ref : nullptr;
+        if (tr) { tr[0] = (int64_t)i_ref; tr[1] = (int64_t)col; tr[2] = hash; tr[3] = -1; tr[4] = 0; tr[5] = 0; }
+        if (std::find(old_dest_prof_ids.begin(), old_dest_prof_ids.end(), dest_prof_id) != old_dest_prof_ids.end()) continue;
+        for (size_t i = 0; i < profile_to_refine->data.size(); ++i)
+            if (dest_prof_id[i]) profile1.AppendRawSequence(*profile_to_refine->data[i]);
+            else profile2.AppendRawSequence(*profile_to_refine->data[i]);
+        profile1.Condense(column_mapping1);
+        profile2.Condense(column_mapping2);
+        profile1.OptimizeGaps();
+        profile2.OptimizeGaps();
+        CProfile* prof = new CProfile(params, s->atp.get());
+        prof->Align(&profile1, &profile2, s->no_threads, 4, &column_mapping1, &column_mapping2);
+        std::sort(prof->data.begin(), prof->data.end(), [](CGappedSequence* p, CGappedSequence* q) { return p->id < q->id; });
+        const bool same = *prof == *profile_to_refine;
+        if (tr) tr[3] = same;
+        if (!same) {
+            prof->CalculateTotalScore();
+            if (tr) tr[5] = prof->total_score;
+            if (prof->total_score >= prev_total_score) {
+                prev_total_score = prof->total_score;
+                std::swap(profile_to_refine, prof);
+                ++n_ref_succ;
+                old_dest_prof_ids.clear();
+                valid_gap_stats = false;
+                if (tr) tr[4] = 1;
+            }
+        } else
+            ++identical;
+        delete prof;
+        old_dest_prof_ids.emplace_back(dest_prof_id);
+        i_succ_ref++;
+    }
+    *width = (uint32_t)profile_to_refine->width;
+    totals[1] = prev_total_score;
+    counts[0] = (uint32_t)i_ref; counts[1] = (uint32_t)i_succ_ref; counts[2] = (uint32_t)n_ref_succ; counts[3] = (uint32_t)identical;
+    if (profile_to_refine->width >= stride) { delete profile_to_refine; return; }   // no room: the caller sees *width >= stride
+    for (auto* gs : profile_to_refine->data) render(gs, refined + (size_t)gs->sequence_no * stride);
+    for (size_t c = 0; c <= profile_to_refine->width; ++c)         // the final profile's tables, (width+1) x 32 each
+        for (size_t r = 0; r < NO_SYMBOLS; ++r) {
+            scores[c * NO_SYMBOLS + r] = profile_to_refine->scores.get_value(c, r);
+            counters[c * NO_SYMBOLS + r] = profile_to_refine->counters.get_value(c, r);
+        }
+    delete profile_to_refine;
 }
 
 } // namespace
@@ -176,73 +254,19 @@ void rr_align_refine(void* h, const char* const* letters, const char* const* ids
     CProfile* profile_to_refine = node[2 * n - 2];
     widths[0] = (uint32_t)profile_to_refine->width;
     for (auto* gs : profile_to_refine->data) render(gs, unrefined + (size_t)gs->sequence_no * stride);
+    refine_loop(s, profile_to_refine, n_refinements, refined, stride, widths + 1, totals, counts, trace, max_trace, scores, counters);
+}
 
-    // msa_refinement.cpp:77, 84-92
-    std::mt19937 rnd_rfn;
-    rnd_rfn.seed(5489u);
-    size_t n_ref = n_refinements;
-    size_t n_seq = profile_to_refine->Size();
-    std::vector<size_t> gap_stats;
-    if (n_ref > 2 * n_seq) n_ref = 2 * n_seq;
-    if (n_ref > 0 && n_ref < 100 && n_seq < 100) n_ref = 100;
-    // :113-209
-    int n_ref_succ = 0, identical = 0;
-    score_t prev_total_score = profile_to_refine->CalculateTotalScore();
-    totals[0] = prev_total_score;
-    std::sort(profile_to_refine->data.begin(), profile_to_refine->data.end(), [](CGappedSequence* p, CGappedSequence* q) { return p->id < q->id; });
-    std::vector<size_t> dest_prof_id;
-    std::vector<std::vector<size_t>> old_dest_prof_ids;
-    std::vector<int> column_mapping1, column_mapping2;
-    size_t i_ref, i_succ_ref;
-    bool valid_gap_stats = false;
-    for (i_ref = i_succ_ref = 0; i_succ_ref < n_ref && i_ref < 20 * n_ref; ++i_ref) {
-        CProfile profile1(params, s->atp.get()), profile2(params, s->atp.get());
-        const size_t col = refine_column(rnd_rfn, profile_to_refine, dest_prof_id, gap_stats, valid_gap_stats);
-        valid_gap_stats = true;
-        uint32_t hash = 2166136261u;
-        for (size_t d : dest_prof_id) hash = (hash ^ (uint32_t)d) * 16777619u;
-        int64_t* tr = i_ref < max_trace ? trace + 6 * i_ref : nullptr;
-        if (tr) { tr[0] = (int64_t)i_ref; tr[1] = (int64_t)col; tr[2] = hash; tr[3] = -1; tr[4] = 0; tr[5] = 0; }
-        if (std::find(old_dest_prof_ids.begin(), old_dest_prof_ids.end(), dest_prof_id) != old_dest_prof_ids.end()) continue;
-        for (size_t i = 0; i < profile_to_refine->data.size(); ++i)
-            if (dest_prof_id[i]) profile1.AppendRawSequence(*profile_to_refine->data[i]);
-            else profile2.AppendRawSequence(*profile_to_refine->data[i]);
-        profile1.Condense(column_mapping1);
-        profile2.Condense(column_mapping2);
-        profile1.OptimizeGaps();
-        profile2.OptimizeGaps();
-        CProfile* prof = new CProfile(params, s->atp.get());
-        prof->Align(&profile1, &profile2, s->no_threads, 4, &column_mapping1, &column_mapping2);
-        std::sort(prof->data.begin(), prof->data.end(), [](CGappedSequence* p, CGappedSequence* q) { return p->id < q->id; });
-        const bool same = *prof == *profile_to_refine;
-        if (tr) tr[3] = same;
-        if (!same) {
-            prof->CalculateTotalScore();
-            if (tr) tr[5] = prof->total_score;
-            if (prof->total_score >= prev_total_score) {
-                prev_total_score = prof->total_score;
-                std::swap(profile_to_refine, prof);
-                ++n_ref_succ;
-                old_dest_prof_ids.clear();
-                valid_gap_stats = false;
-                if (tr) tr[4] = 1;
-            }
-        } else
-            ++identical;
-        delete prof;
-        old_dest_prof_ids.emplace_back(dest_prof_id);
-        i_succ_ref++;
-    }
-    widths[1] = (uint32_t)profile_to_refine->width;
-    totals[1] = prev_total_score;
-    counts[0] = (uint32_t)i_ref; counts[1] = (uint32_t)i_succ_ref; counts[2] = (uint32_t)n_ref_succ; counts[3] = (uint32_t)identical;
-    for (auto* gs : profile_to_refine->data) render(gs, refined + (size_t)gs->sequence_no * stride);
-    for (size_t c = 0; c <= profile_to_refine->width; ++c)         // the final profile's tables, (width+1) x 32 each
-        for (size_t r = 0; r < NO_SYMBOLS; ++r) {
-            scores[c * NO_SYMBOLS + r] = profile_to_refine->scores.get_value(c, r);
-            counters[c * NO_SYMBOLS + r] = profile_to_refine->counters.get_value(c, r);
-        }
-    delete profile_to_refine;
+// RefineAlignment of the alignment given as n NUL-terminated rows of letters ('-': gap) with FASTA ids `ids` (sequence
+// number = index), built as rr_total_score builds it; outputs as rr_align_refine's, widths[0] = the input's width.
+void rr_refine_rows(void* h, const char* const* rows, const char* const* ids, uint32_t n, uint32_t n_refinements, char* refined,
+                    uint32_t stride, uint32_t* widths, int64_t* totals, uint32_t* counts, int64_t* trace, uint32_t max_trace,
+                    int64_t* scores, int32_t* counters)
+{
+    auto* s = static_cast<Session*>(h);
+    CProfile* p = from_rows(s, rows, n, ids);
+    widths[0] = (uint32_t)p->width;
+    refine_loop(s, p, n_refinements, refined, stride, widths + 1, totals, counts, trace, max_trace, scores, counters);
 }
 
 } // extern "C"

@@ -5,7 +5,9 @@
   edits): the independent check of the device's k_ref_score_* and k_ref_optimize, which use other formulations;
 * the reference behind oracle/ref_refine_harness.cpp (oracle/_ref/libfamsa_ref_refine.so): its own CalculateTotalScore
   and OptimizeGaps on given rows, and its progressive alignment followed by the restated RefineAlignment loop, with the
-  per-try trace and the final profile's tables."""
+  per-try trace and the final profile's tables; and its RefineAlignment loop on a given alignment;
+* total_score_rows: CalculateTotalScore vectorised, with a third formulation of the gap-open count, for widths the
+  reference's (width+1)^2 / 2 tables and the restatement above cannot reach."""
 from __future__ import annotations
 
 import ctypes as C
@@ -21,6 +23,12 @@ def have_ref() -> bool:
     return os.path.exists(SO)
 
 
+def have_refine_rows() -> bool:
+    """The harness has rr_refine_rows (a library built where the reference's sources could not be read may be one
+    carried over from an older revision of ref_refine_harness.cpp, which has only the other entry points)."""
+    return have_ref() and hasattr(_load(), "rr_refine_rows")
+
+
 def _load():
     global _lib
     if _lib is None:
@@ -34,6 +42,10 @@ def _load():
         lib.rr_align_refine.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_char_p,
                                         C.c_char_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
                                         C.c_void_p, C.c_void_p]
+        if hasattr(lib, "rr_refine_rows"):
+            lib.rr_refine_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_char_p,
+                                           C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
+                                           C.c_void_p, C.c_void_p]
         _lib = lib
     return _lib
 
@@ -84,13 +96,40 @@ class RefRefine:
                                  widths.ctypes.data, totals.ctypes.data, counts.ctypes.data, trace.ctypes.data, max_trace,
                                  scores.ctypes.data, counters.ctypes.data)
 
-        def rows(buf, w):
-            return [buf.raw[i * stride:i * stride + w].decode() for i in range(n)]
-        return dict(unrefined=rows(unref, int(widths[0])), refined=rows(ref, int(widths[1])), width=int(widths[1]),
-                    prev_total=int(totals[0]), total=int(totals[1]),
-                    counts=dict(n_tries=int(counts[0]), n_realigned=int(counts[1]), n_accepted=int(counts[2]),
-                                n_identical=int(counts[3])),
-                    trace=trace[:int(counts[0])], scores=scores[:int(widths[1]) + 1], counters=counters[:int(widths[1]) + 1])
+        return _result(n, stride, unref, ref, widths, totals, counts, trace, scores, counters)
+
+    def refine_rows(self, rows: list[str], ids: list[str], n_refinements: int = 100) -> dict:
+        """RefineAlignment of a given alignment (rows of letters, '-' for a gap; row i is sequence i with FASTA id ids[i]).
+        Returns align_refine's dict, with 'unrefined' the rows given.  The refined width must stay below 2 W + 2 (room
+        the rows are given); a refinement that grows wider raises."""
+        n, w = len(rows), len(rows[0])
+        stride = 2 * w + 2
+        ref = C.create_string_buffer(n * stride)
+        widths = np.zeros(2, dtype=np.uint32)
+        totals = np.zeros(2, dtype=np.int64)
+        counts = np.zeros(4, dtype=np.uint32)
+        max_trace = 20 * max(100, min(n_refinements, 2 * n))
+        trace = np.zeros((max_trace, 6), dtype=np.int64)
+        scores = np.zeros((stride + 1, 32), dtype=np.int64)
+        counters = np.zeros((stride + 1, 32), dtype=np.int32)
+        self.lib.rr_refine_rows(self.h, _strs(rows), _strs(ids), n, n_refinements, ref, stride, widths.ctypes.data,
+                                totals.ctypes.data, counts.ctypes.data, trace.ctypes.data, max_trace, scores.ctypes.data,
+                                counters.ctypes.data)
+        if widths[1] >= stride:
+            raise RuntimeError(f"refined width {int(widths[1])} leaves no room in rows of {stride} bytes")
+        out = _result(n, stride, None, ref, widths, totals, counts, trace, scores, counters)
+        out["unrefined"] = list(rows)
+        return out
+
+
+def _result(n, stride, unref, ref, widths, totals, counts, trace, scores, counters) -> dict:
+    def rows(buf, w):
+        return [buf.raw[i * stride:i * stride + w].decode() for i in range(n)]
+    return dict(unrefined=rows(unref, int(widths[0])) if unref is not None else None, refined=rows(ref, int(widths[1])),
+                width=int(widths[1]), prev_total=int(totals[0]), total=int(totals[1]),
+                counts=dict(n_tries=int(counts[0]), n_realigned=int(counts[1]), n_accepted=int(counts[2]),
+                            n_identical=int(counts[3])),
+                trace=trace[:int(counts[0])], scores=scores[:int(widths[1]) + 1], counters=counters[:int(widths[1]) + 1])
 
 
 # ------------------------------------------------------------------------------------------------ numpy restatements
@@ -166,6 +205,49 @@ def total_score(rows: np.ndarray, counters: np.ndarray, sm: np.ndarray, gaps) ->
     n_ext -= n_open
     n_text -= n_topen
     return score + n_ext * ge + n_open * go + n_text * te + n_topen * to
+
+
+def run_bounds(rows: np.ndarray):
+    """(row, first column, last column) of every gap run of an n x W alignment, 1-based columns, as three int64 arrays."""
+    g = np.zeros((rows.shape[0], rows.shape[1] + 2), dtype=np.int8)
+    g[:, 1:-1] = rows == GAP
+    d = np.diff(g, axis=1)
+    r0, s = np.nonzero(d == 1)                                # a run starts in column s + 1 (1-based)
+    r1, e = np.nonzero(d == -1)                               # ... and ends in column e
+    assert np.array_equal(r0, r1)
+    return r0.astype(np.int64), s.astype(np.int64) + 1, e.astype(np.int64)
+
+
+def total_score_rows(rows: np.ndarray, counters: np.ndarray, sm: np.ndarray, gaps, chunk: int = 1 << 12) -> int:
+    """CalculateTotalScore (profile.cpp:1368-1542) of an n x W alignment with counters (W+1) x 32, vectorised and in
+    O(W + runs x n) for any width.  Column terms from the counters in exact int64: symbol pairs (upper triangle of sm,
+    and the diagonal x C(n_k, 2)), residue x internal-gap and residue x terminal-gap pairs.  Gap opens by a third
+    formulation: a run [s, e] of one row opens against every row that has a residue somewhere in [s, e] (the rows
+    without one are exactly those whose run through s contains [s, e]); per-row prefix sums of residues answer that.
+    The run is terminal when s == 1 or e == W."""
+    go, ge, to, te = (int(x) for x in gaps)
+    rows = np.asarray(rows)
+    n, W = rows.shape
+    cnt = np.asarray(counters, dtype=np.int64)[1:W + 1]
+    s64 = np.asarray(sm, dtype=np.int64)[:24, :24]
+    k = cnt[:, :24]
+    pair = int(((k @ np.triu(s64, 1)) * k).sum()) + int(((k * (k - 1) // 2) @ np.diag(s64)).sum())
+    ng, nt = cnt[:, GO] + cnt[:, GE], cnt[:, TO] + cnt[:, TE]
+    ns = n - ng - nt
+    n_ext, n_text = int((ns * ng).sum()), int((ns * nt).sum())
+    pre = np.zeros((n, W + 1), dtype=np.int32)                # pre[r, c]: residues of row r in columns 1..c
+    np.cumsum(rows != GAP, axis=1, out=pre[:, 1:])
+    _, s, e = run_bounds(rows)
+    n_open = n_topen = 0
+    for lo in range(0, len(s), chunk):
+        ss, ee = s[lo:lo + chunk], e[lo:lo + chunk]
+        v = (pre[:, ee] > pre[:, ss - 1]).sum(axis=0).astype(np.int64)
+        term = (ss == 1) | (ee == W)
+        n_topen += int(v[term].sum())
+        n_open += int(v[~term].sum())
+    n_ext -= n_open
+    n_text -= n_topen
+    return pair + n_ext * ge + n_open * go + n_text * te + n_topen * to
 
 
 def containing_runs_brute(rows: np.ndarray) -> int:

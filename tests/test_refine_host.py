@@ -1,7 +1,8 @@
 """CPU checks of famsa_prof_refine's checkers: the numpy restatements of CalculateTotalScore and OptimizeGaps
 (tests/refine_oracle.py) against the reference's own functions on random gapped alignments, the formulation of the
 gap-open count against brute force, the reference defect of a missing length-1 run, and the restated RefineAlignment loop
-of oracle/ref_refine_harness.cpp (its per-try trace agrees with its counts)."""
+of oracle/ref_refine_harness.cpp (its per-try trace agrees with its counts, and its two entry points run one loop);
+the vectorised total_score_rows against both totals."""
 from __future__ import annotations
 
 import numpy as np
@@ -79,6 +80,43 @@ def test_total_score_restatement_equals_reference(kind, seed):
     assert ro.total_score(a, counters(a, sm, g), sm, g) == want
 
 
+@pytest.mark.parametrize("kind", KINDS + ["no_len1"])
+@pytest.mark.parametrize("seed", range(6))
+def test_total_score_rows_equals_restatement_and_reference(kind, seed):
+    """The vectorised count (a run opens against every row with a residue inside it) is the same total."""
+    a = alignment(kind, seed)
+    g, sm = rc.scoring(a.shape[0])
+    cn = counters(a, sm, g)
+    got = ro.total_score_rows(a, cn, sm, g)
+    assert got == ro.total_score(a, cn, sm, g)
+    if ro.have_ref() and kind != "no_len1":
+        ref = ro.RefRefine(sm, g)
+        assert got == ref.total_score([rc.to_letters(r) for r in a])
+        ref.close()
+
+
+def long_run_alignments():
+    """Runs longer than 256 columns (one block of k_ref_score_runs' suffix scan), terminal runs at column 1 and W."""
+    import refine_shapes as S
+    yield S.alignment(4, 600, seed=1, runs=[(1, 10, 266), (2, 1, 300)])
+    yield S.alignment(3, 400, seed=2, runs=[(1, 1, 399)])
+    yield S.alignment(3, 400, seed=3, runs=[(1, 2, 400)])
+    yield S.alignment(6, 900, seed=4, runs=[(1, 1, 1), (2, 900, 900), (3, 300, 899), (4, 2, 258)])
+
+
+@need_ref
+@pytest.mark.parametrize("case", range(4))
+def test_total_score_rows_equals_reference_on_long_runs(case):
+    a = list(long_run_alignments())[case]
+    assert max(ln for row in a for ln, _ in ro.gap_runs(row)) > 256 and has_len1(a)
+    g, sm = rc.scoring(a.shape[0])
+    ref = ro.RefRefine(sm, g)
+    want = ref.total_score([rc.to_letters(r) for r in a])
+    ref.close()
+    cn = counters(a, sm, g)
+    assert ro.total_score_rows(a, cn, sm, g) == ro.total_score(a, cn, sm, g) == want
+
+
 @need_ref
 @pytest.mark.parametrize("kind", KINDS)
 @pytest.mark.parametrize("seed", range(6))
@@ -131,3 +169,18 @@ def test_trace_matches_counts(n, flags):
         acc = t[t[:, 4] == 1]
         assert (len(acc) == 0 and r["total"] == r["prev_total"]) or acc[-1, 5] == r["total"]
     assert c["n_realigned"] == 100 or c["n_tries"] == 2000
+
+
+@pytest.mark.skipif(not ro.have_refine_rows(), reason="the harness library has no rr_refine_rows: rebuild oracle/refine.mk")
+def test_refine_rows_is_the_loop_of_align_refine():
+    """rr_refine_rows on the unrefined rows of rr_align_refine gives the same refinement, try for try."""
+    n = 30
+    g, sm = rc.scoring(n)
+    ref = ro.RefRefine(sm, g)
+    ids = [f"s{i}" for i in range(n)]
+    a = ref.align_refine(rc.family(n, 60, seed=4), dp_cases.random_tree(n, np.random.default_rng(4)), ids=ids)
+    b = ref.refine_rows(a["unrefined"], ids)
+    ref.close()
+    assert b["refined"] == a["refined"] and b["counts"] == a["counts"] and (b["prev_total"], b["total"]) == (a["prev_total"], a["total"])
+    assert np.array_equal(b["trace"], a["trace"]) and np.array_equal(b["scores"], a["scores"])
+    assert np.array_equal(b["counters"], a["counters"])
