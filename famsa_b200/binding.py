@@ -6,6 +6,8 @@ import os
 
 import numpy as np
 
+from . import profiles, seqio
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 
 EXPORTED_SYMBOLS = [
@@ -16,7 +18,7 @@ EXPORTED_SYMBOLS = [
     "famsa_lcs_last_timing", "famsa_dp_align_batch", "famsa_dp_align_batch_device", "famsa_dp_last_timing",
     "famsa_prof_set_scoring", "famsa_prof_put", "famsa_prof_merge_batch", "famsa_prof_get", "famsa_prof_drop",
     "famsa_prof_last_timing", "famsa_prof_stats", "famsa_prof_align_tree", "famsa_prof_tree_paths",
-    "famsa_prof_refine", "famsa_prof_refined_rows",
+    "famsa_prof_refine", "famsa_prof_refined_rows", "famsa_prof_put_rows",
 ]
 
 PROF_LEAF = 0x80000000            # FAMSA_PROF_LEAF
@@ -55,6 +57,7 @@ class RefineStats(C.Structure):
 
 REFINE_NO_GAP_OPT = 1        # -dgo
 REFINE_NO_TOTAL_SCORE = 2    # -dsp
+PUT_ROWS_FROM_TEXT = 1       # famsa_prof_put_rows: the profile the reference builds from rows read as text
 
 
 class FamsaError(RuntimeError):
@@ -119,6 +122,7 @@ def load_library() -> C.CDLL:
     lib.famsa_lcs_last_timing.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(u64)]
     lib.famsa_prof_set_scoring.argtypes = [vp, vp]
     lib.famsa_prof_put.argtypes = [vp, vp, u32, vp]
+    lib.famsa_prof_put_rows.argtypes = [vp, vp, u32, u32, vp, C.c_int, C.POINTER(u32)]
     lib.famsa_prof_merge_batch.argtypes = [vp, vp, u32, vp, vp, vp, vp, u64]
     lib.famsa_prof_get.argtypes = [vp, u32, C.POINTER(u32), C.POINTER(u32), vp, vp]
     lib.famsa_prof_drop.argtypes = [vp, vp, u32]
@@ -433,6 +437,42 @@ class Engine:
         ids = np.zeros(max(n, 1), dtype=np.uint32)
         self._check(self.lib.famsa_prof_put(self.h, C.byref(arr), n, _ptr(ids)))
         return [int(x) for x in ids[:n]]
+
+    def prof_put_rows(self, rows, gaps, from_text: bool = False) -> int:
+        """famsa_prof_put_rows: a resident profile from a finished alignment, rows (n, width) uint8 codes with GAP = 30
+        (seqio.encode_gapped), in the order the profile keeps them.  from_text: FAMSA_PUT_ROWS_FROM_TEXT, the profile
+        (width - 1 columns) the reference builds from rows read as text.  Returns its id."""
+        r = np.ascontiguousarray(rows, dtype=np.uint8)
+        if r.ndim != 2:
+            raise ValueError("rows must be an (n_rows, width) array")
+        g = np.ascontiguousarray(gaps, dtype=np.int64)
+        pid = C.c_uint32()
+        self._check(self.lib.famsa_prof_put_rows(self.h, _ptr(r), r.shape[0], r.shape[1], _ptr(g), PUT_ROWS_FROM_TEXT if from_text else 0,
+                                                 C.byref(pid)))
+        return pid.value
+
+    def align_profiles(self, rows1: list[str], rows2: list[str], gaps) -> dict:
+        """FAMSA's profile-profile mode (famsa in1 in2 out, CFAMSA::alignProfiles without its refinement): the two
+        alignments' rows as text, gaps = the rescaled costs of adjustParams(n1 + n2).  Needs prof_set_scoring.
+        Returns dict(order, rows, width, total, swapped, variant, path, merged_id): output row k is rows[k], input row
+        order[k] of rows1 + rows2 with its letters as given; merged_id is the merged resident profile (the caller drops it)."""
+        for k, rows in enumerate((rows1, rows2), 1):
+            if not rows or any(len(r) != len(rows[0]) for r in rows):        # famsa.cpp:83-89 "Incorrect profile"
+                raise ValueError(f"alignment {k} is empty or its rows differ in length")
+        ids = [self.prof_put_rows(np.stack([seqio.encode_gapped(r) for r in rows1]), gaps, from_text=True)]
+        try:
+            ids.append(self.prof_put_rows(np.stack([seqio.encode_gapped(r) for r in rows2]), gaps, from_text=True))
+            (merged,), (res,) = self.prof_merge_batch([tuple(ids)], gaps, [(len(rows1[0]) - 1, len(rows2[0]) - 1)])
+        except Exception:
+            for i in ids:                        # whichever of the inputs is still resident
+                try:
+                    self.prof_drop([i])
+                except FamsaError:
+                    pass
+            raise
+        order, rows = profiles.rows_after_merge(rows1, rows2, res["path"], res["swapped"], from_text=True)
+        return dict(order=order, rows=rows, width=len(rows[0]), total=res["total"], swapped=res["swapped"],
+                    variant=res["variant"], path=res["path"], merged_id=merged)
 
     def prof_merge_batch(self, merges, gaps, widths):
         """merges: list of (child1, child2) -- resident ids or PROF_LEAF | sequence id; widths: matching list of

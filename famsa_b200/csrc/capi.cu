@@ -678,6 +678,16 @@ int famsa_prof_put(famsa_ctx* ctx, const famsa_dp_profile* profiles, uint32_t n,
     return fb::prof_put(ctx, profiles, n, ids_out);
 }
 
+int famsa_prof_put_rows(famsa_ctx* ctx, const uint8_t* rows, uint32_t n_rows, uint32_t width, const int64_t gaps[4], int flags,
+                        uint32_t* id_out)
+{
+    return entry(ctx, nullptr, nullptr, [&]() -> int {
+        if (!rows || !gaps || !id_out) { set_error("NULL argument"); return FAMSA_E_INVALID; }
+        if (flags & ~FAMSA_PUT_ROWS_FROM_TEXT) { set_error("famsa_prof_put_rows: unknown flags"); return FAMSA_E_INVALID; }
+        return FAMSA_OK;
+    }, [&](cudaStream_t) { return fb::prof_put_rows(ctx, rows, n_rows, width, gaps, flags, id_out); });
+}
+
 int famsa_prof_merge_batch(famsa_ctx* ctx, const famsa_prof_merge* merges, uint32_t n, const int64_t gaps[4],
                            uint32_t* merged_ids_out, famsa_dp_result* results, uint8_t* path_buf, uint64_t path_cap)
 {

@@ -124,6 +124,7 @@ struct ProfEntry {
     int slab = -1;
     bool live = false;
     bool pending = false;          // produced by a batch the host has not collected yet: the real width lives in d_widths[id]
+    bool text_col = false;         // FAMSA_PUT_ROWS_FROM_TEXT: counters hold column width + 1 too (DpJobExt::x1 / x2)
     uint32_t gen = 0;              // bumped whenever the id is handed out again
 };
 // One queued batch of merges (prof_launch ... prof_collect)
@@ -329,5 +330,6 @@ int prof_refine(famsa_ctx* ctx, uint32_t root_id, const uint8_t* rows, uint32_t 
                 uint32_t n_refinements, int flags, uint32_t* refined_id, uint32_t* width_out, int64_t* total_score,
                 famsa_refine_stats* stats);
 int prof_refined_rows(famsa_ctx* ctx, uint8_t* rows, uint64_t cap);
+int prof_put_rows(famsa_ctx* ctx, const uint8_t* rows, uint32_t n_rows, uint32_t width, const int64_t gaps[4], int flags, uint32_t* id_out);
 void refine_release(famsa_ctx* ctx);
 } // namespace fb

@@ -290,6 +290,8 @@ __device__ __forceinline__ void prep_body(const DpParams& P, uint32_t jid)
                 }
             }
         }
+        // ProfProf's orientation also counts a set-aside column past the width (DpJobExt::x1 / x2), one row per lane
+        if (var == 2 && tid < 32 && (side ? J.x2 : J.x1)) nz += cnt[(size_t)(w + 1) * 32 + tid] != 0;
         for (int o = 16; o; o >>= 1) {
             nz += __shfl_xor_sync(0xffffffffu, nz, o);
             const unsigned long long x = __shfl_xor_sync(0xffffffffu, smax, o);
@@ -1429,7 +1431,8 @@ static int job_dev(const famsa_dp_job* jobs, const DpJobExt* ext, uint32_t k, Dp
     }
     d = DpJobDev{reinterpret_cast<const long long*>(j.p1.scores), j.p1.counters, reinterpret_cast<const long long*>(j.p2.scores), j.p2.counters,
                  j.p1.width, j.p1.card, j.p2.width, j.p2.card,
-                 ext ? ext[k].w1_src : nullptr, ext ? ext[k].w2_src : nullptr, ext ? ext[k].w_dst : nullptr, 0, 0, 0, 0};
+                 ext ? ext[k].w1_src : nullptr, ext ? ext[k].w2_src : nullptr, ext ? ext[k].w_dst : nullptr, 0, 0, 0, 0,
+                 ext ? ext[k].x1 : 0u, ext ? ext[k].x2 : 0u};
     return FAMSA_OK;
 }
 

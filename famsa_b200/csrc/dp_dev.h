@@ -32,12 +32,16 @@ struct DpJobDev {
     const uint32_t* w1_src; const uint32_t* w2_src;
     uint32_t* w_dst;                                               // receives the merged width (path length), or kWidthBad
     unsigned long long path_off, dirs_off, scratch_off, t_off;     // t_off: offset of the job's skewed direction bytes
+    uint32_t x1, x2;                                               // counter columns past the width that ProfProf's orientation counts
 };
 
 // host-side companion of famsa_dp_job for dp_run_device
 struct DpJobExt {
     const uint32_t* w1_src; const uint32_t* w2_src;
     uint32_t* w_dst;
+    // 1 for a profile built from rows read as text (FAMSA_PUT_ROWS_FROM_TEXT): its counters keep the set-aside last
+    // column, which the reference's get_num_of_non_zeros counts (CalculateCountersScores sizes them gapped_size + 1)
+    uint32_t x1 = 0, x2 = 0;
 };
 
 struct DpFusedPlan { unsigned long long scratch_bytes, skew_bytes, path_bytes, cells; };

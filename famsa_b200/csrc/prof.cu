@@ -177,7 +177,7 @@ void place(ProfState& P, uint32_t id, int slab, size_t* cursor, uint32_t width, 
     char* base = static_cast<char*>(P.slabs[slab].p) + *cursor;
     e.scores = reinterpret_cast<long long*>(base);
     e.counters = reinterpret_cast<int*>(base + ((size_t)width + 1) * kRows * sizeof(long long));
-    e.width = width; e.card = card; e.slab = slab; e.live = true; e.pending = false;
+    e.width = width; e.card = card; e.slab = slab; e.live = true; e.pending = false; e.text_col = false;
     *cursor += table_bytes(width);                                  // multiple of 384: keeps 128-byte alignment
     ++P.slabs[slab].live;
     ++P.n_live;
@@ -322,6 +322,7 @@ static int prof_resolve(famsa_ctx* ctx, const famsa_prof_merge* merges, uint32_t
                 const ProfEntry& e = P.entries[c];
                 p.scores = reinterpret_cast<const int64_t*>(e.scores); p.counters = e.counters; p.width = e.width; p.card = e.card;
                 if (e.pending) src = P.d_widths.as<uint32_t>() + c;
+                (side ? B.ext[k].x2 : B.ext[k].x1) = e.text_col;
             }
         }
     }

@@ -15,6 +15,9 @@
 //   k_ref_run_ends, k_ref_score_cols, CalculateTotalScore (profile.cpp:1368-1542) from the candidate's merged counters
 //   k_ref_score_runs, k_ref_gapstats  and rows, and the candidate's gap counts (GetGapStats)                -> host, sync 3
 // DESIGN.md §4d has the reasoning, the launch list and the formulation of the gap-open count.
+//
+// famsa_prof_put_rows (a resident profile from a finished alignment, CFAMSA::alignProfiles' inputs) builds its tables with
+// the same k_ref_row_ends + k_ref_tables pass (gapped_tables) as a try's two sides.
 #include <algorithm>
 #include <chrono>
 #include <cstring>
@@ -460,6 +463,22 @@ __global__ void k_ref_transpose(const uint8_t* __restrict__ in, uint8_t* __restr
 
 unsigned blocks(size_t n, unsigned t) { return (unsigned)((n + t - 1) / t); }
 
+// CalculateCountersScores (profile.cpp:101-235) of the column-major gapped rows of S's sides 0..n_sides-1 into T: the one
+// builder of tables from gapped rows, for a refinement try's two sides and for famsa_prof_put_rows' one alignment (side 0,
+// with S.n[1] = 0).  first / last: scratch of S.n[0] + S.n[1] words each.
+int gapped_tables(famsa_ctx* ctx, cudaStream_t st, const Sides& S, int n_sides, uint32_t* first, uint32_t* last,
+                  const SideTables& T, const int64_t g[4])
+{
+    const uint32_t nmax = n_sides > 1 ? std::max(S.n[0], S.n[1]) : S.n[0], wmax = n_sides > 1 ? std::max(S.w[0], S.w[1]) : S.w[0];
+    k_ref_row_ends<<<dim3(blocks(nmax, 128), n_sides), 128, 0, st>>>(S, first, last);
+    FB_CUDA(cudaGetLastError());
+    k_ref_tables<<<dim3(wmax + 1, n_sides), kRT, 0, st>>>(S, first, last, T, ctx->prof.d_sm.as<long long>(), (long long)g[0],
+                                                         (long long)g[1], (long long)g[2], (long long)g[3]);
+    FB_CUDA(cudaGetLastError());
+    ctx->launches += 2;
+    return FAMSA_OK;
+}
+
 // The device state of one famsa_prof_refine call.
 struct Run {
     famsa_ctx* ctx;
@@ -676,9 +695,7 @@ static int refine_run(famsa_ctx* ctx, uint32_t root_id, const uint8_t* rows, uin
         SideTables T{{P.entries[ids[1]].scores, P.entries[ids[0]].scores}, {P.entries[ids[1]].counters, P.entries[ids[0]].counters}};
         FB_TRY(X.launch(k_ref_condense, blocks((size_t)n * W, kRT), kRT, 0, (const uint8_t*)R.d_cur.as<uint8_t>(), n, W,
                         (const uint8_t*)X.dest, (const int*)C0.map, (const uint32_t*)X.ridx, SD));
-        FB_TRY(X.launch(k_ref_row_ends, dim3(blocks(std::max(n0, n1), 128), 2), 128, 0, SD, X.first, X.last));
-        FB_TRY(X.launch(k_ref_tables, dim3(std::max(w0, w1) + 1, 2), kRT, 0, SD, (const uint32_t*)X.first, (const uint32_t*)X.last, T,
-                        (const long long*)P.d_sm.as<long long>(), (long long)gaps[0], (long long)gaps[1], (long long)gaps[2], (long long)gaps[3]));
+        FB_TRY(gapped_tables(ctx, st, SD, 2, X.first, X.last, T, gaps));
         if (opt_gaps) FB_TRY(X.launch(k_ref_optimize, 2, kOptT, 0, SD, X.otype, X.orf, X.ors));
 
         // Align + ConstructProfile through the merge path of famsa_prof_merge_batch; the sides are consumed
@@ -785,6 +802,91 @@ int prof_refined_rows(famsa_ctx* ctx, uint8_t* rows, uint64_t cap)
     ++ctx->launches;
     FB_CUDA(cudaMemcpyAsync(rows, R.d_cand.p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
     FB_CUDA(cudaStreamSynchronize(ctx->stream));
+    return FAMSA_OK;
+}
+
+// famsa_prof_put_rows: the rows go up into stream-ordered scratch of the call's own (refine's state stays as it is), are
+// turned column-major and gapped_tables builds the new entry's tables.
+static int put_rows_run(famsa_ctx* ctx, const uint8_t* rows, uint32_t n, uint32_t width, const int64_t gaps[4], uint32_t id)
+{
+    cudaStream_t st = ctx->stream;
+    Layout L;
+    const size_t cells = (size_t)n * width;
+    const size_t o_raw = L.add(cells), o_cm = L.add(cells), o_first = L.add(4 * (size_t)n), o_last = L.add(4 * (size_t)n);
+    char* blob = nullptr;
+    const cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&blob), L.end, st);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        set_error("famsa_prof_put_rows: cudaMallocAsync(" + std::to_string(L.end) + ") failed: " + cudaGetErrorString(e));
+        return FAMSA_E_NOMEM;
+    }
+    uint8_t* raw = reinterpret_cast<uint8_t*>(blob + o_raw);
+    uint8_t* cm = reinterpret_cast<uint8_t*>(blob + o_cm);
+    auto body = [&]() -> int {
+        FB_CUDA(cudaMemcpyAsync(raw, rows, cells, cudaMemcpyHostToDevice, st));
+        k_ref_transpose<<<dim3(blocks(width, 32), blocks(n, 32)), dim3(32, 8), 0, st>>>(raw, cm, n, width);
+        FB_CUDA(cudaGetLastError());
+        ++ctx->launches;
+        Sides S{};
+        S.rows[0] = cm; S.n[0] = n; S.w[0] = width;
+        const ProfEntry& E = ctx->prof.entries[id];
+        const SideTables T{{E.scores, nullptr}, {E.counters, nullptr}};
+        return gapped_tables(ctx, st, S, 1, reinterpret_cast<uint32_t*>(blob + o_first), reinterpret_cast<uint32_t*>(blob + o_last), T, gaps);
+    };
+    int rc = body();
+    const cudaError_t f = cudaFreeAsync(blob, st);
+    if (rc == FAMSA_OK && f != cudaSuccess) { set_error(std::string("famsa_prof_put_rows: cudaFreeAsync failed: ") + cudaGetErrorString(f)); rc = FAMSA_E_CUDA; }
+    return rc;
+}
+
+int prof_put_rows(famsa_ctx* ctx, const uint8_t* rows, uint32_t n, uint32_t width, const int64_t gaps[4], int flags, uint32_t* id_out)
+{
+    if (!ctx->prof.has_scoring) { set_error("famsa_prof_put_rows: famsa_prof_set_scoring has not been called"); return FAMSA_E_STATE; }
+    const bool from_text = flags & FAMSA_PUT_ROWS_FROM_TEXT;
+    if (!n || width < (from_text ? 2u : 1u)) {
+        set_error("famsa_prof_put_rows: an alignment of " + std::to_string(n) + " x " + std::to_string(width) + " is empty");
+        return FAMSA_E_INVALID;
+    }
+    const uint32_t kept = from_text ? width - 1 : width;          // the columns of the profile
+    for (uint32_t r = 0; r < n; ++r) {
+        bool residue = false, gap = false;
+        for (uint32_t c = 0; c < width; ++c) {
+            const uint8_t v = rows[(size_t)r * width + c];
+            if (v != kGAP && v >= kNAA) { set_error("famsa_prof_put_rows: row " + std::to_string(r) + " holds code " + std::to_string(v)); return FAMSA_E_INVALID; }
+            residue |= v != kGAP;
+            gap |= v == kGAP && c < kept;
+        }
+        if (!residue) { set_error("famsa_prof_put_rows: row " + std::to_string(r) + " has no residue"); return FAMSA_E_INVALID; }
+        // a one-row profile is aligned as a sequence whose residues are its columns (AlignSeqSeq / AlignSeqProf)
+        if (n == 1 && gap) { set_error("famsa_prof_put_rows: a one-row alignment cannot hold a gap"); return FAMSA_E_INVALID; }
+    }
+    uint32_t id;
+    FB_TRY(prof_new(ctx, 1, &width, &n, &id));
+    const int rc = put_rows_run(ctx, rows, n, width, gaps, id);
+    if (rc != FAMSA_OK) {
+        // the new entry does not stay resident; the error message of the failure is kept
+        const std::string msg = get_error();
+        cudaStreamSynchronize(ctx->stream);
+        prof_drop(ctx, &id, 1);
+        set_error(msg);
+        return rc;
+    }
+    // FAMSA_PUT_ROWS_FROM_TEXT: the reference's profile is these tables without their last column (see the header).  Its
+    // counters still hold that column, with the residues alone (no terminal gap reaches past the width), and ProfProf's
+    // orientation counts it (DpJobExt::x1 / x2).
+    if (from_text) {
+        ProfEntry& E = ctx->prof.entries[id];
+        const cudaError_t z = cudaMemsetAsync(E.counters + (size_t)width * kRows + kNAA, 0, (kRows - kNAA) * sizeof(int), ctx->stream);
+        if (z != cudaSuccess) {
+            set_error(std::string("famsa_prof_put_rows: cudaMemsetAsync failed: ") + cudaGetErrorString(z));
+            cudaStreamSynchronize(ctx->stream);
+            prof_drop(ctx, &id, 1);
+            return FAMSA_E_CUDA;
+        }
+        --E.width;
+        E.text_col = true;
+    }
+    *id_out = id;
     return FAMSA_OK;
 }
 

@@ -281,6 +281,64 @@ inline TreeAlignment AlignTree(Context& ctx, const std::vector<std::pair<int, in
     return out;
 }
 
+// CFAMSA::alignProfiles (msa.cpp:675-718) without its RefineAlignment: the two alignments' profiles as the reference builds
+// them from rows read as text (famsa_prof_put_rows with FAMSA_PUT_ROWS_FROM_TEXT: each profile leaves out its last column)
+// and one unbanded merge.  rows: codes 0..23 or GAP = 30, every row of an alignment as long as its first.  Needs
+// famsa_prof_set_scoring.  gaps1 / gaps2: the GapRuns FinalizeGaps applies to rows1's / rows2's members (the row profile's
+// H runs, the column profile's V runs); the last column of every input row stays apart and ends its merged row.
+// order[k]: input row (k < n1: rows1[k], else rows2[k - n1]) of merged row k -- the column profile's rows, then the row
+// profile's (ConstructProfile, profile.cpp:992-993).  merged_id: the merged resident profile, the caller's to drop.
+struct ProfileAlignment {
+    AlignResult merge;
+    uint32_t merged_id = 0;
+    std::vector<std::pair<uint32_t, uint32_t>> gaps1, gaps2;
+    std::vector<uint32_t> order;
+};
+inline ProfileAlignment AlignProfiles(Context& ctx, const std::vector<std::vector<uint8_t>>& rows1,
+                                      const std::vector<std::vector<uint8_t>>& rows2, const int64_t gaps[4])
+{
+    const std::vector<std::vector<uint8_t>>* in[2] = {&rows1, &rows2};
+    uint32_t ids[2], widths[2];
+    int n_put = 0;
+    try {
+        for (int s = 0; s < 2; ++s) {
+            const auto& rows = *in[s];
+            if (rows.empty()) throw std::runtime_error("Incorrect profile");      // famsa.cpp:83-89
+            std::vector<uint8_t> flat;
+            for (const auto& r : rows) {
+                if (r.size() != rows.front().size()) throw std::runtime_error("Incorrect profile");
+                flat.insert(flat.end(), r.begin(), r.end());
+            }
+            check(famsa_prof_put_rows(ctx.get(), flat.data(), (uint32_t)rows.size(), (uint32_t)rows.front().size(), gaps,
+                                      FAMSA_PUT_ROWS_FROM_TEXT, &ids[s]));
+            widths[s] = (uint32_t)rows.front().size() - 1;
+            ++n_put;
+        }
+    } catch (...) {
+        if (n_put) famsa_prof_drop(ctx.get(), ids, (uint32_t)n_put);
+        throw;
+    }
+    const famsa_prof_merge m{ids[0], ids[1]};
+    famsa_dp_result r{};
+    std::vector<uint8_t> path((size_t)widths[0] + widths[1]);
+    ProfileAlignment out;
+    check(famsa_prof_merge_batch(ctx.get(), &m, 1, gaps, &out.merged_id, &r, path.data(), path.size()));
+    out.merge.path.assign(path.begin() + r.path_offset, path.begin() + r.path_offset + r.path_len);
+    out.merge.total_score = r.total_score;
+    std::copy(r.last, r.last + 3, out.merge.last);
+    out.merge.swapped = r.swapped != 0;
+    out.merge.variant = r.variant;
+    const uint32_t n1 = (uint32_t)rows1.size(), n2 = (uint32_t)rows2.size();
+    auto row_runs = GapRuns(out.merge.path, 1), col_runs = GapRuns(out.merge.path, 2);
+    out.gaps1 = out.merge.swapped ? col_runs : row_runs;
+    out.gaps2 = out.merge.swapped ? row_runs : col_runs;
+    const uint32_t col_first = out.merge.swapped ? 0 : n1, col_n = out.merge.swapped ? n1 : n2;
+    const uint32_t row_first = out.merge.swapped ? n1 : 0, row_n = out.merge.swapped ? n2 : n1;
+    for (uint32_t i = 0; i < col_n; ++i) out.order.push_back(col_first + i);
+    for (uint32_t i = 0; i < row_n; ++i) out.order.push_back(row_first + i);
+    return out;
+}
+
 // UPGMA<distance>::run (UPGMA.cpp:39-51) on the device: the n - 1 merges, tree_structure's internal-node part
 inline std::vector<std::pair<int, int>> UPGMATree(Context& ctx, Distance measure, bool modified)
 {

@@ -60,6 +60,41 @@ def tables_from_rows(rows: np.ndarray, score_matrix: np.ndarray, gaps) -> tuple[
     return scores, cnt.astype(np.int32), card
 
 
+def rows_after_merge(rows1: list[str], rows2: list[str], path, swapped: bool, from_text: bool = False) -> tuple[list[int], list[str]]:
+    """The rows of the profile a merge of two alignments builds: ConstructProfile ends with data = profile2->data;
+    append(profile1->data) (profile.cpp:992-993), profile2 being the DP's column profile, so the column side's rows come
+    first, each side in its input order.  swapped: famsa_dp_result.swapped (the DP's rows are rows2).  A merged row is its
+    input row with the path's gap columns inserted: H (1) inserts a gap column into the row side, V (2) into the column
+    side (FinalizeGaps, profile.cpp:1053-1104).  Letters are kept as given, so lower case and non-standard letters
+    survive as CGappedSequence::uppercase / extra_symbols make them survive.
+    from_text: the profiles were built from rows read as text (famsa_prof_put_rows' FAMSA_PUT_ROWS_FROM_TEXT, what
+    famsa in1 in2 out does): the path covers all but the last column of each side, and that column ends every merged row.
+    Returns (order, rows): output row k is input row order[k] of rows1 + rows2."""
+    if from_text:
+        order, rows = rows_after_merge([r[:-1] for r in rows1], [r[:-1] for r in rows2], path, swapped)
+        return order, [r + (rows1[k] if k < len(rows1) else rows2[k - len(rows1)])[-1] for k, r in zip(order, rows)]
+    p = np.asarray(path, dtype=np.uint8)
+    n1 = len(rows1)
+    row_side, col_side = (1, 0) if swapped else (0, 1)
+
+    def insert(rows: list[str], skip: int) -> list[str]:
+        if not rows:
+            return []
+        a = np.frombuffer("".join(rows).encode("latin-1"), dtype=np.uint8).reshape(len(rows), -1)
+        take = p != skip
+        if int(take.sum()) != a.shape[1]:
+            raise ValueError(f"the path consumes {int(take.sum())} columns of a side {a.shape[1]} wide")
+        out = np.full((a.shape[0], len(p)), ord("-"), dtype=np.uint8)
+        out[:, take] = a
+        return [r.tobytes().decode("latin-1") for r in out]
+
+    sides = (rows1, rows2)
+    merged = {row_side: insert(sides[row_side], 1), col_side: insert(sides[col_side], 2)}
+    base = (0, n1)
+    order = [base[col_side] + i for i in range(len(sides[col_side]))] + [base[row_side] + i for i in range(len(sides[row_side]))]
+    return order, merged[col_side] + merged[row_side]
+
+
 def synth_alignment(card: int, width: int, rng, gap_frac: float = 0.12) -> np.ndarray:
     """A plausible aligned block: a consensus with per-row substitutions and random gap runs; every column
     keeps at least one residue (as any real profile does)."""

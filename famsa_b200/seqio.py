@@ -11,6 +11,7 @@ import numpy as np
 ALPHABET = "ARNDCQEGHILKMFPSTWYVBZX*"
 UNKNOWN = 22
 N_VALID = 20
+GAP = 30                                 # a gap in the rows of a finished alignment (src/core/defs.h)
 
 _LUT = np.full(256, UNKNOWN, dtype=np.int8)
 for _i, _ch in enumerate(ALPHABET):
@@ -23,6 +24,13 @@ def encode(seq: str) -> np.ndarray:
     raw = np.frombuffer(seq.encode("ascii", "replace"), dtype=np.uint8)
     raw = raw[raw != ord("-")]
     return _LUT[raw]
+
+
+def encode_gapped(row: str) -> np.ndarray:
+    """One row of a finished alignment as famsa_prof_put_rows and famsa_prof_refine take it (uint8): '-' -> GAP,
+    every other letter as encode() maps it (CGappedSequence's constructor, sequence.cpp:214-272)."""
+    raw = np.frombuffer(row.encode("ascii", "replace"), dtype=np.uint8)
+    return np.where(raw == ord("-"), GAP, _LUT[raw]).astype(np.uint8)
 
 
 def decode(codes: np.ndarray) -> str:

@@ -340,6 +340,38 @@ int famsa_prof_set_scoring(famsa_ctx* ctx, const int64_t score_matrix[24 * 24]);
 /* Uploads n host profiles (same layout as famsa_dp_profile for famsa_dp_align_batch) as resident ones. */
 int famsa_prof_put(famsa_ctx* ctx, const famsa_dp_profile* profiles, uint32_t n, uint32_t* ids_out);
 
+/* A resident profile from a finished (gapped) alignment: CProfile::AppendRawSequence for every row +
+ * CalculateCountersScores (src/core/profile.cpp:101-235, :329-350), as CFAMSA::alignProfiles builds its two inputs
+ * (src/msa.cpp:675-691): no Condense, no OptimizeGaps, all-gap columns kept.  rows: n_rows x width bytes, row-major, in the
+ * order AppendRawSequence sees them; each byte a residue code 0..23 or GAP = 30 (no GUARD), as for famsa_prof_refine.
+ * gaps = {gap_open, gap_ext, gap_term_open, gap_term_ext}, the rescaled costs the merge will also use (for the
+ * profile-profile mode: adjustParams(n1 + n2), src/famsa.cpp:94).  *id_out: an ordinary resident profile of card n_rows,
+ * for famsa_prof_merge_batch, famsa_prof_get, famsa_prof_drop, or as a famsa_prof_refine root.  Its width is `width`, and
+ * width - 1 with FAMSA_PUT_ROWS_FROM_TEXT.
+ * FAMSA_PUT_ROWS_FROM_TEXT: the profile the reference builds from rows read as text.  Such a CGappedSequence already starts
+ * with GUARD (sequence.cpp:234), so AppendRawSequence sets the profile's width to gapped_size - 1 (profile.cpp:333-336)
+ * while CalculateCounters still reads every residue and internal gap of the whole row: the profile is the flag-free one
+ * without its last column (a gap run up to a residue in that column stays an internal one).  CalculateCountersScores
+ * still sizes the counters gapped_size + 1, so they keep that column's residues, and the ProfProf orientation test
+ * (get_num_of_non_zeros, profile.cpp:283) counts them: the entry keeps them too and the merge counts them the same way.
+ * The DP never aligns that column; FinalizeGaps keeps it at the end of every merged row.  This is what
+ * famsa in1 in2 out computes.
+ * FAMSA's profile-profile mode is two of these calls with FAMSA_PUT_ROWS_FROM_TEXT and one
+ * famsa_prof_merge_batch({id1, id2}); the merged rows are the column profile's rows, then the row profile's
+ * (famsa_dp_result.swapped tells which is which), each with the path's gap columns inserted (INTEGRATION.md).
+ * Does not touch the state of famsa_prof_refine: famsa_prof_refined_rows still returns the last refinement's rows.
+ * FAMSA_E_STATE without famsa_prof_set_scoring; FAMSA_E_INVALID for NULL pointers, unknown flags, n_rows == 0 or width == 0
+ * (width < 2 with FAMSA_PUT_ROWS_FROM_TEXT), a code that is neither < 24 nor 30, a row without a residue (CalculateCounters
+ * would read symbols[0] of an empty sequence) and a one-row alignment with a gap in a column the profile keeps (with
+ * FAMSA_PUT_ROWS_FROM_TEXT a gap in the last column is allowed): the reference aligns a one-row profile
+ * as a sequence and its Seq* cell loops read the residues as the columns (src/core/profile_seq.cpp:32-33,176), so a gap
+ * makes them read past the sequence; FAMSA_E_NOMEM when an allocation fails.  Nothing the call made stays resident after
+ * an error, and the context stays usable. */
+#define FAMSA_PUT_ROWS_FROM_TEXT 1
+
+int famsa_prof_put_rows(famsa_ctx* ctx, const uint8_t* rows, uint32_t n_rows, uint32_t width, const int64_t gaps[4],
+                        int flags, uint32_t* id_out);
+
 /* Aligns and merges n independent pairs.  Resident children are consumed (as ComputeAlignment deletes
  * them, msa.cpp:406-407).  merged_ids_out[k] is the resident id of merge k's profile (width =
  * results[k].path_len, card = sum of the children's).  results/path_buf as in famsa_dp_align_batch
