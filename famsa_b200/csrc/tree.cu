@@ -674,12 +674,30 @@ struct UnionFind {
     }
 };
 
+// Development knobs, read on every call.  FAMSA_TREE_MAX_BLOCKS=<k> caps the cooperative grids of k_prim, k_upgma and
+// k_nj at k blocks, so that a few thousand sequences reach what otherwise only sets above ~135 k do on an H100: threads
+// that own several sequences, warps that scan dozens of NJ rows.  It only ever lowers a grid; unset, 0 or unparsable
+// changes nothing.  FAMSA_TREE_DEBUG: one `[coop] <kernel> n=<n> blocks=<grid>` line per cooperative launch on stderr.
+static uint32_t coop_cap(uint32_t nblk)
+{
+    const char* e = getenv("FAMSA_TREE_MAX_BLOCKS");
+    if (!e) return nblk;
+    char* end = nullptr;
+    const long k = strtol(e, &end, 10);
+    if (end == e || *end || k <= 0) return nblk;
+    return (uint32_t)std::min<long>(nblk, k);
+}
+static void coop_debug(const char* kernel, uint32_t n, uint32_t nblk)
+{
+    if (getenv("FAMSA_TREE_DEBUG")) fprintf(stderr, "[coop] %s n=%u blocks=%u\n", kernel, n, nblk);
+}
+
 // Blocks of 1024 threads for a cooperative kernel over n items: all co-resident, no more than the items need
 static int coop_blocks(famsa_ctx* ctx, const void* fn, uint32_t n, uint32_t& nblk)
 {
     int per_sm = 0;
     FB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, 1024, 0));
-    nblk = std::max(1u, std::min((uint32_t)(ctx->sm_count * std::max(per_sm, 1)), (n + 1023) / 1024));
+    nblk = coop_cap(std::max(1u, std::min((uint32_t)(ctx->sm_count * std::max(per_sm, 1)), (n + 1023) / 1024)));
     return FAMSA_OK;
 }
 
@@ -877,6 +895,7 @@ static int mst(famsa_ctx* ctx, int kind, bool parallel, std::vector<MstEdge>& ed
     PrimCand* a_cand = S.d_tree_cand.as<PrimCand>();
     void* args[] = {&a_tri, &a_eb, &a_n, &a_len, &a_pow, &a_kind, &a_sidx, &a_side, &d_state, &d_vis,
                     &a_cand, &d_from, &d_to, &d_dist, &d_order};
+    coop_debug(kSlink ? "k_prim<1>" : "k_prim<0>", n, nblk);
     FB_CUDA(cudaLaunchCooperativeKernel((void*)k_prim<kSlink>, dim3(nblk), dim3(1024), args, 0, st));
     ctx->launches++;
     if (n > 1) {
@@ -987,6 +1006,7 @@ int lcs_upgma(famsa_ctx* ctx, int kind, int modified, int32_t* h_tree, const voi
         uint32_t a_n = n;
         unsigned long long* a_cand = S.d_tree_cand.as<unsigned long long>();
         void* args[] = {&d_dist, &a_n, &d_mind, &d_nn, &d_node, &a_cand, &d_tree, &d_status};
+        coop_debug(modified ? "k_upgma<1>" : "k_upgma<0>", n, nblk);
         FB_CUDA(cudaLaunchCooperativeKernel(fn, dim3(nblk), dim3(1024), args, 0, st));
         ctx->launches++;
     }
@@ -1030,11 +1050,12 @@ int lcs_nj(famsa_ctx* ctx, int kind, int32_t* h_tree)
     // the scan of the first merges reads the whole triangle: blocks for every 64 rows, all co-resident
     int per_sm = 0;
     FB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void*)k_nj, 1024, 0));
-    const uint32_t nblk = std::max(1u, std::min((uint32_t)(ctx->sm_count * std::max(per_sm, 1)), (n + 63) / 64));
+    const uint32_t nblk = coop_cap(std::max(1u, std::min((uint32_t)(ctx->sm_count * std::max(per_sm, 1)), (n + 63) / 64)));
     FB_TRY(S.d_tree_cand.reserve(sizeof(NjCand) * nblk));
     uint32_t a_n = n;
     NjCand* a_cand = S.d_tree_cand.as<NjCand>();
     void* args[] = {&d_dist, &d_half, &a_n, &d_s0, &d_s1, &d_node0, &d_node1, &d_map, &d_misc, &a_cand, &d_tree, &d_status};
+    coop_debug("k_nj", n, nblk);
     FB_CUDA(cudaLaunchCooperativeKernel((const void*)k_nj, dim3(nblk), dim3(1024), args, 0, st));
     ctx->launches++;
     int status = 0;
