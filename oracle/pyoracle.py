@@ -166,6 +166,11 @@ def have_ref() -> bool:
     return os.path.exists(REF_SO)
 
 
+def have_ref_set_scores() -> bool:
+    """Is the reference library built with ref_profile_set_scores (RefDp.set_scores)?"""
+    return have_ref() and hasattr(ref(), "ref_profile_set_scores")
+
+
 def ref() -> C.CDLL:
     global _ref
     if _ref is None:
@@ -208,6 +213,8 @@ def ref() -> C.CDLL:
         lib.ref_profile_total_score.argtypes = [vp]
         lib.ref_profile_total_score.restype = i64
         lib.ref_profile_tables.argtypes = [vp, vp, vp]
+        if hasattr(lib, "ref_profile_set_scores"):       # absent from a library built before the harness had it
+            lib.ref_profile_set_scores.argtypes = [vp, vp]
         lib.ref_profile_row.argtypes = [vp, u32, vp]
         lib.ref_profile_row.restype = C.c_int
         lib.ref_profile_align.argtypes = [vp, vp, vp, C.c_int]
@@ -283,6 +290,13 @@ class RefDp:
         cn = np.zeros((w + 1, 32), dtype=np.int32)
         self.lib.ref_profile_tables(p, _p(sc), _p(cn))
         return sc, cn, int(self.lib.ref_profile_card(p))
+
+    def set_scores(self, p, scores: np.ndarray):
+        """Replaces the profile's score table (counters untouched): Align then runs on the given scores."""
+        w = self.lib.ref_profile_width(p)
+        s = np.ascontiguousarray(scores, dtype=np.int64)
+        assert s.shape == (w + 1, 32)
+        self.lib.ref_profile_set_scores(p, _p(s))
 
     def rows(self, p) -> dict[int, str]:
         w = self.lib.ref_profile_width(p)

@@ -359,6 +359,15 @@ void ref_profile_tables(void* p, int64_t* scores, int32_t* counters)
         }
 }
 
+// overwrites the profile's scores ((width+1) x 32 int64, layout as ref_profile_tables), counters untouched: CProfile::Align
+// reads the stored table, so crafted scores steer its path while ConstructProfile still works on the real counters
+void ref_profile_set_scores(void* p, const int64_t* scores)
+{
+    auto* q = static_cast<CProfile*>(p);
+    for (size_t c = 0; c <= q->width; ++c)
+        for (size_t r = 0; r < NO_SYMBOLS; ++r) q->scores.set_value(c, r, scores[c * NO_SYMBOLS + r]);
+}
+
 // gapped row i of the profile (width characters + NUL) and its sequence number
 int ref_profile_row(void* p, uint32_t i, char* out)
 {
