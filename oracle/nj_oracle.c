@@ -1,5 +1,5 @@
 /* oracle/nj_oracle.c -- a plain C restatement of NeighborJoining<>::computeTree (src/tree/NeighborJoining.cpp:33-118 of
- * FAMSA v2.5.0).  TEST INFRASTRUCTURE ONLY: built by oracle/nj.mk into oracle/libnj_oracle.so.
+ * FAMSA v2.5.0).  TEST INFRASTRUCTURE ONLY: built by oracle/Makefile into oracle/libnj_oracle.so.
  *
  * ISO C float arithmetic (FLT_EVAL_METHOD 0, compiled with -ffp-contract=off), so every operation is rounded on its own
  * as in the reference's build, which has no FMA to contract into.  Where the reference would go on with a step that has

@@ -1,5 +1,10 @@
-"""ctypes access to the checkers: oracle/liboracle.so (our C restatement) and
-oracle/_ref/libfamsa_ref.so (the unmodified reference behind oracle/ref_harness.cpp).
+"""ctypes access to the checkers: the only module that opens one of their libraries.
+
+  oracle/liboracle.so, oracle/libnj_oracle.so   our C restatements (oracle/*_oracle.c)
+  oracle/_ref/libfamsa_ref*.so                  the unmodified reference behind oracle/ref_*harness.cpp
+
+lib(name) opens a library of LIBS once; have(name, symbol) says whether it is there and has an entry point.  The wrappers
+of liboracle.so and libfamsa_ref.so live here; tests/{nj,slink,dist_export,refine}_oracle.py wrap the others.
 
 TEST INFRASTRUCTURE ONLY -- importable from tests/, __graft_entry__.smoke() and bench.py's
 cpu_baseline / --impl reference legs; never from famsa_b200/.
@@ -13,43 +18,123 @@ import subprocess
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-ORACLE_SO = os.path.join(_HERE, "liboracle.so")
-REF_SO = os.path.join(_HERE, "_ref", "libfamsa_ref.so")
+
+vp, cp, i32, u32, i64, u64 = C.c_void_p, C.c_char_p, C.c_int, C.c_uint32, C.c_int64, C.c_uint64
+f32, f64 = C.c_float, C.c_double
+
+# name: (file under oracle/, built on demand by `make -C oracle` when missing, {entry point: (restype, argtypes)}).
+# Only oracle/Makefile builds the _ref/ libraries, and only where the reference's sources are.
+LIBS = {
+    "oracle": ("liboracle.so", True, {
+        "lcs_oracle_rows": (None, [vp, vp, vp, vp, u32, vp, u32, vp]),
+        "lcs_oracle_triangle": (None, [vp, vp, vp, u32, u32, vp]),
+        "lcs_oracle_transform_f64": (f64, [i32, u32, u32, u32]),
+        "lcs_oracle_transform_f32": (f32, [i32, u32, u32, u32]),
+        "lcs_oracle_transform_tri_f32": (None, [i32, vp, i32, vp, u32, vp]),
+        "upgma_oracle_tree": (i32, [vp, u32, i32, i32, i32, vp, vp]),
+        "dp_oracle_align": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+        "dp_oracle_construct": (i32, [vp, vp, vp, u32, vp, vp, vp, vp, vp, vp, vp]),
+    }),
+    "nj_oracle": ("libnj_oracle.so", True, {
+        "nj_oracle_tree": (i32, [vp, u32, vp, vp]),
+    }),
+    "ref": ("_ref/libfamsa_ref.so", False, {
+        "ref_seqset_create": (vp, [vp, u32]),
+        "ref_seqset_destroy": (None, [vp]),
+        "ref_seqset_len": (u32, [vp, u32]),
+        "ref_seqset_codes": (None, [vp, u32, vp]),
+        "ref_lcs_row_prefix": (None, [vp, u32, u32, vp, i32]),
+        "ref_lcs_row_ids": (None, [vp, u32, vp, u32, vp, i32]),
+        "ref_lcs_triangle_mt": (f64, [vp, u32, u32, i32, i32, vp, vp]),
+        "ref_mst_prim_tree": (None, [vp, i32, vp]),
+        "ref_mst_to_dendogram": (None, [i32, vp, vp, vp, vp, vp]),
+        "ref_upgma_tree": (None, [vp, i32, i32, vp]),
+        "ref_upgma_tree_from_distances": (None, [vp, i32, i32, vp]),
+        "ref_transform_f64": (f64, [i32, u32, u32, u32]),
+        "ref_transform_f32": (f32, [i32, u32, u32, u32]),
+        "ref_dp_create": (vp, [i32, i32, i32]),
+        "ref_dp_destroy": (None, [vp]),
+        "ref_dp_gaps": (None, [vp, vp]),
+        "ref_dp_set_gaps": (None, [vp, vp]),
+        "ref_dp_score_matrix": (None, [vp, vp]),
+        "ref_profile_create": (vp, [vp, vp, vp, u32]),
+        "ref_profile_leaf": (vp, [vp, cp, i32]),
+        "ref_profile_destroy": (None, [vp]),
+        "ref_profile_width": (u32, [vp]),
+        "ref_profile_card": (u32, [vp]),
+        "ref_profile_total_score": (i64, [vp]),
+        "ref_profile_tables": (None, [vp, vp, vp]),
+        "ref_profile_set_scores": (None, [vp, vp]),
+        "ref_profile_row": (i32, [vp, u32, vp]),
+        "ref_profile_align": (vp, [vp, vp, vp, i32]),
+        "ref_profile_construct": (vp, [vp, vp, vp, vp, vp, i32]),
+        "ref_dp_align_pairs_mt": (f64, [vp, vp, vp, u32, i32, vp]),
+        "ref_align_tree_mt": (f64, [vp, vp, u32, vp, i32, vp, vp, vp, vp, u32]),
+    }),
+    "ref_dist": ("_ref/libfamsa_ref_dist.so", False, {
+        "ref_dist_export": (i32, [vp, vp, u32, i32, i32, i32, cp, i32]),
+        "ref_num2str_f32": (u64, [vp, u64, vp]),
+    }),
+    "ref_slink": ("_ref/libfamsa_ref_slink.so", False, {
+        "ref_slink_tree": (i32, [vp, u32, i32, i32, vp]),
+    }),
+    "ref_nj": ("_ref/libfamsa_ref_nj.so", False, {
+        "ref_nj_tree": (i32, [vp, u32, i32, vp, vp]),
+        "ref_nj_tree_from_distances": (i32, [vp, i32, i32, vp]),
+    }),
+    "ref_refine": ("_ref/libfamsa_ref_refine.so", False, {
+        "rr_create": (vp, [vp, vp, i32, i32]),
+        "rr_destroy": (None, [vp]),
+        "rr_total_score": (i64, [vp, vp, u32]),
+        "rr_optimize_gaps": (None, [vp, vp, u32, cp]),
+        "rr_align_refine": (None, [vp, vp, vp, u32, vp, u32, cp, cp, u32, vp, vp, vp, vp, u32, vp, vp]),
+        "rr_refine_rows": (None, [vp, vp, vp, u32, u32, cp, u32, vp, vp, vp, vp, u32, vp, vp]),
+    }),
+}
+_libs: dict[str, C.CDLL] = {}
 
 
-def build(quiet: bool = True):
-    """(Re)build the checkers: liboracle.so always, _ref only where /root/reference exists."""
-    subprocess.run(["make", "-C", _HERE, "-j8", "all"], check=True,
-                   stdout=subprocess.DEVNULL if quiet else None)
+def _path(name: str) -> str:
+    return os.path.join(_HERE, LIBS[name][0])
+
+
+def lib(name: str) -> C.CDLL:
+    """The library LIBS[name], opened once.  A _ref/ library carried over from a build of an older revision (where the
+    reference's sources could not be read to rebuild it) may lack newer entry points: only those the file exports are
+    declared, and have(name, symbol) tells which."""
+    if name not in _libs:
+        _, on_demand, entry_points = LIBS[name]
+        if on_demand and not os.path.exists(_path(name)):
+            subprocess.run(["make", "-C", _HERE, "-j8", "all"], check=True, stdout=subprocess.DEVNULL)
+        dll = C.CDLL(_path(name))
+        for symbol, (restype, argtypes) in entry_points.items():
+            if hasattr(dll, symbol):
+                getattr(dll, symbol).restype = restype
+                getattr(dll, symbol).argtypes = argtypes
+        _libs[name] = dll
+    return _libs[name]
+
+
+def have(name: str, symbol: str | None = None) -> bool:
+    """Whether the file of LIBS[name] is there and, given `symbol`, exports that entry point."""
+    return os.path.exists(_path(name)) and (symbol is None or hasattr(lib(name), symbol))
+
+
+def have_ref() -> bool:
+    return have("ref")
+
+
+def have_ref_set_scores() -> bool:
+    """Is the reference library built with ref_profile_set_scores (RefDp.set_scores)?"""
+    return have("ref", "ref_profile_set_scores")
+
+
+def ref() -> C.CDLL:
+    return lib("ref")
 
 
 def _p(a):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
-
-
-_oracle = None
-
-
-def oracle() -> C.CDLL:
-    global _oracle
-    if _oracle is None:
-        if not os.path.exists(ORACLE_SO):
-            build()
-        lib = C.CDLL(ORACLE_SO)
-        vp, u32 = C.c_void_p, C.c_uint32
-        lib.lcs_oracle_rows.argtypes = [vp, vp, vp, vp, u32, vp, u32, vp]
-        lib.lcs_oracle_triangle.argtypes = [vp, vp, vp, u32, u32, vp]
-        lib.lcs_oracle_transform_f64.argtypes = [C.c_int, u32, u32, u32]
-        lib.lcs_oracle_transform_f64.restype = C.c_double
-        lib.lcs_oracle_transform_f32.argtypes = [C.c_int, u32, u32, u32]
-        lib.lcs_oracle_transform_f32.restype = C.c_float
-        lib.lcs_oracle_transform_tri_f32.argtypes = [C.c_int, vp, C.c_int, vp, u32, vp]
-        lib.upgma_oracle_tree.argtypes = [vp, u32, C.c_int, C.c_int, C.c_int, vp, vp]
-        lib.upgma_oracle_tree.restype = C.c_int
-        lib.dp_oracle_align.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
-        lib.dp_oracle_construct.argtypes = [vp, vp, vp, u32, vp, vp, vp, vp, vp, vp, vp]
-        _oracle = lib
-    return _oracle
 
 
 class DpProfile(C.Structure):
@@ -59,7 +144,7 @@ class DpProfile(C.Structure):
 def dp_align(scores1, counters1, card1, scores2, counters2, card2, gaps, score_matrix=None):
     """Oracle version of CProfile::Align + traceback.  scores: (W+1,32) int64, counters: (W+1,32) int32.
     Returns dict(path uint8[], total, last(3), swapped, variant, dirs (WR+1, WC+1) uint8)."""
-    lib = oracle()
+    dll = lib("oracle")
     s1 = np.ascontiguousarray(scores1, dtype=np.int64); c1 = np.ascontiguousarray(counters1, dtype=np.int32)
     s2 = np.ascontiguousarray(scores2, dtype=np.int64); c2 = np.ascontiguousarray(counters2, dtype=np.int32)
     w1, w2 = s1.shape[0] - 1, s2.shape[0] - 1
@@ -71,7 +156,7 @@ def dp_align(scores1, counters1, card1, scores2, counters2, card2, gaps, score_m
     path = np.zeros(w1 + w2 + 1, dtype=np.uint8)
     plen = C.c_uint32(); total = C.c_int64(); sw = C.c_int(); var = C.c_int()
     last = np.zeros(3, dtype=np.int64)
-    lib.dp_oracle_align(C.byref(p1), C.byref(p2), _p(g), _p(sm), _p(dirs), _p(path), C.byref(plen), _p(last),
+    dll.dp_oracle_align(C.byref(p1), C.byref(p2), _p(g), _p(sm), _p(dirs), _p(path), C.byref(plen), _p(last),
                         C.byref(total), C.byref(sw), C.byref(var))
     wr, wc = (w2, w1) if sw.value else (w1, w2)
     return dict(path=path[:plen.value].copy(), total=total.value, last=last, swapped=bool(sw.value),
@@ -83,7 +168,7 @@ def dp_construct(rows_prof, cols_prof, path, gaps):
     DP matrix's row / column profile (i.e. after the orientation swap); path = forward direction bytes.
     Returns (scores (W+1,32) int64, counters (W+1,32) int32, gap runs of the row profile's members (m,2),
     gap runs of the column profile's members (m,2)) -- runs are (first merged column, length)."""
-    lib = oracle()
+    dll = lib("oracle")
     s1 = np.ascontiguousarray(rows_prof[0], dtype=np.int64); c1 = np.ascontiguousarray(rows_prof[1], dtype=np.int32)
     s2 = np.ascontiguousarray(cols_prof[0], dtype=np.int64); c2 = np.ascontiguousarray(cols_prof[1], dtype=np.int32)
     p1 = DpProfile(s1.ctypes.data, c1.ctypes.data, s1.shape[0] - 1, int(rows_prof[2]))
@@ -94,7 +179,7 @@ def dp_construct(rows_prof, cols_prof, path, gaps):
     os_ = np.zeros((w + 1, 32), dtype=np.int64); oc = np.zeros((w + 1, 32), dtype=np.int32)
     g1 = np.zeros((max(w, 1), 2), dtype=np.uint32); g2 = np.zeros((max(w, 1), 2), dtype=np.uint32)
     n1 = C.c_uint32(); n2 = C.c_uint32()
-    rc = lib.dp_oracle_construct(C.byref(p1), C.byref(p2), _p(path), w, _p(g), _p(os_), _p(oc), _p(g1), C.byref(n1),
+    rc = dll.dp_oracle_construct(C.byref(p1), C.byref(p2), _p(path), w, _p(g), _p(os_), _p(oc), _p(g1), C.byref(n1),
                                  _p(g2), C.byref(n2))
     if rc:
         raise ValueError(f"dp_oracle_construct: path does not span the two profiles (rc={rc})")
@@ -102,28 +187,28 @@ def dp_construct(rows_prof, cols_prof, path, gaps):
 
 
 def lcs_rows(codes, offsets, lens, ref_ids, col_ids=None, n_col=None) -> np.ndarray:
-    lib = oracle()
+    dll = lib("oracle")
     ref = np.ascontiguousarray(ref_ids, dtype=np.uint32)
     cols = None if col_ids is None else np.ascontiguousarray(col_ids, dtype=np.uint32)
     n_col = (len(lens) if n_col is None else n_col) if cols is None else len(cols)
     out = np.zeros(max(len(ref) * n_col, 1), dtype=np.uint32)
-    lib.lcs_oracle_rows(_p(codes), _p(offsets), _p(lens), _p(ref), len(ref), _p(cols), n_col, _p(out))
+    dll.lcs_oracle_rows(_p(codes), _p(offsets), _p(lens), _p(ref), len(ref), _p(cols), n_col, _p(out))
     return out[:len(ref) * n_col].reshape(len(ref), n_col)
 
 
 def lcs_triangle(codes, offsets, lens, row_begin=0, row_end=None) -> np.ndarray:
-    lib = oracle()
+    dll = lib("oracle")
     row_end = len(lens) if row_end is None else row_end
     f = lambda r: r * (r - 1) // 2 if r else 0
     size = f(row_end) - f(row_begin)
     out = np.zeros(max(size, 1), dtype=np.uint32)
-    lib.lcs_oracle_triangle(_p(codes), _p(offsets), _p(lens), row_begin, row_end, _p(out))
+    dll.lcs_oracle_triangle(_p(codes), _p(offsets), _p(lens), row_begin, row_end, _p(out))
     return out[:size]
 
 
 def transform(kind: int, lcs: int, len1: int, len2: int, double=True) -> float:
-    lib = oracle()
-    return float((lib.lcs_oracle_transform_f64 if double else lib.lcs_oracle_transform_f32)(kind, lcs, len1, len2))
+    dll = lib("oracle")
+    return float((dll.lcs_oracle_transform_f64 if double else dll.lcs_oracle_transform_f32)(kind, lcs, len1, len2))
 
 
 def transform_triangle(kind: int, lcs_tri: np.ndarray, lens) -> np.ndarray:
@@ -136,7 +221,7 @@ def transform_triangle(kind: int, lcs_tri: np.ndarray, lens) -> np.ndarray:
     n = len(ln)
     assert t.size == n * (n - 1) // 2
     out = np.empty(max(t.size, 1), dtype=np.float32)
-    oracle().lcs_oracle_transform_tri_f32(kind, _p(t), t.dtype.itemsize, _p(ln), n, _p(out))
+    lib("oracle").lcs_oracle_transform_tri_f32(kind, _p(t), t.dtype.itemsize, _p(ln), n, _p(out))
     return out[:t.size]
 
 
@@ -154,88 +239,18 @@ def upgma_tree(dist_tri: np.ndarray, n: int, modified: bool = False, avg_mode: i
     assert d.size == n * (n - 1) // 2
     out = np.zeros((max(n - 1, 1), 2), dtype=np.int32)
     done = C.c_uint32()
-    rc = oracle().upgma_oracle_tree(_p(d), n, int(modified), avg_mode, int(fresh_cache), _p(out), C.byref(done))
+    rc = lib("oracle").upgma_oracle_tree(_p(d), n, int(modified), avg_mode, int(fresh_cache), _p(out), C.byref(done))
     return rc, out[:done.value]
 
 
 # ------------------------------------------------------------------ the real reference
-_ref = None
-
-
-def have_ref() -> bool:
-    return os.path.exists(REF_SO)
-
-
-def have_ref_set_scores() -> bool:
-    """Is the reference library built with ref_profile_set_scores (RefDp.set_scores)?"""
-    return have_ref() and hasattr(ref(), "ref_profile_set_scores")
-
-
-def ref() -> C.CDLL:
-    global _ref
-    if _ref is None:
-        lib = C.CDLL(REF_SO)
-        vp, u32 = C.c_void_p, C.c_uint32
-        lib.ref_seqset_create.argtypes = [vp, u32]
-        lib.ref_seqset_create.restype = vp
-        lib.ref_seqset_destroy.argtypes = [vp]
-        lib.ref_seqset_len.argtypes = [vp, u32]
-        lib.ref_seqset_len.restype = u32
-        lib.ref_seqset_codes.argtypes = [vp, u32, vp]
-        lib.ref_lcs_row_prefix.argtypes = [vp, u32, u32, vp, C.c_int]
-        lib.ref_lcs_row_ids.argtypes = [vp, u32, vp, u32, vp, C.c_int]
-        lib.ref_lcs_triangle_mt.argtypes = [vp, u32, u32, C.c_int, C.c_int, vp, vp]
-        lib.ref_lcs_triangle_mt.restype = C.c_double
-        lib.ref_mst_prim_tree.argtypes = [vp, C.c_int, vp]
-        lib.ref_mst_to_dendogram.argtypes = [C.c_int, vp, vp, vp, vp, vp]
-        lib.ref_upgma_tree.argtypes = [vp, C.c_int, C.c_int, vp]
-        lib.ref_upgma_tree_from_distances.argtypes = [vp, C.c_int, C.c_int, vp]
-        lib.ref_transform_f64.argtypes = [C.c_int, u32, u32, u32]
-        lib.ref_transform_f64.restype = C.c_double
-        lib.ref_transform_f32.argtypes = [C.c_int, u32, u32, u32]
-        lib.ref_transform_f32.restype = C.c_float
-        i64 = C.c_int64
-        lib.ref_dp_create.argtypes = [C.c_int, C.c_int, C.c_int]
-        lib.ref_dp_create.restype = vp
-        lib.ref_dp_destroy.argtypes = [vp]
-        lib.ref_dp_gaps.argtypes = [vp, vp]
-        lib.ref_dp_set_gaps.argtypes = [vp, vp]
-        lib.ref_dp_score_matrix.argtypes = [vp, vp]
-        lib.ref_profile_create.argtypes = [vp, vp, vp, u32]
-        lib.ref_profile_create.restype = vp
-        lib.ref_profile_leaf.argtypes = [vp, C.c_char_p, C.c_int]
-        lib.ref_profile_leaf.restype = vp
-        lib.ref_profile_destroy.argtypes = [vp]
-        lib.ref_profile_width.argtypes = [vp]
-        lib.ref_profile_width.restype = u32
-        lib.ref_profile_card.argtypes = [vp]
-        lib.ref_profile_card.restype = u32
-        lib.ref_profile_total_score.argtypes = [vp]
-        lib.ref_profile_total_score.restype = i64
-        lib.ref_profile_tables.argtypes = [vp, vp, vp]
-        if hasattr(lib, "ref_profile_set_scores"):       # absent from a library built before the harness had it
-            lib.ref_profile_set_scores.argtypes = [vp, vp]
-        lib.ref_profile_row.argtypes = [vp, u32, vp]
-        lib.ref_profile_row.restype = C.c_int
-        lib.ref_profile_align.argtypes = [vp, vp, vp, C.c_int]
-        lib.ref_profile_align.restype = vp
-        lib.ref_profile_construct.argtypes = [vp, vp, vp, vp, vp, C.c_int]
-        lib.ref_profile_construct.restype = vp
-        lib.ref_dp_align_pairs_mt.argtypes = [vp, vp, vp, u32, C.c_int, vp]
-        lib.ref_dp_align_pairs_mt.restype = C.c_double
-        lib.ref_align_tree_mt.argtypes = [vp, vp, u32, vp, C.c_int, vp, vp, vp, vp, u32]
-        lib.ref_align_tree_mt.restype = C.c_double
-        _ref = lib
-    return _ref
-
-
 def mst_to_dendogram(edge_from, edge_to, edge_dist, prim_orders) -> np.ndarray:
     """The reference's own mst_to_dendogram on external MST edges (Prim order)."""
     n = len(prim_orders)
     f = np.ascontiguousarray(edge_from, dtype=np.int32); t = np.ascontiguousarray(edge_to, dtype=np.int32)
     d = np.ascontiguousarray(edge_dist, dtype=np.float64); o = np.ascontiguousarray(prim_orders, dtype=np.int32)
     out = np.zeros((2 * n - 1, 2), dtype=np.int32)
-    ref().ref_mst_to_dendogram(n, _p(f), _p(t), _p(d), _p(o), _p(out))
+    lib("ref").ref_mst_to_dendogram(n, _p(f), _p(t), _p(d), _p(o), _p(out))
     return out
 
 
@@ -243,7 +258,7 @@ def upgma_tree_from_distances(tri: np.ndarray, n: int, modified: bool = False) -
     """The reference's UPGMA agglomeration (computeTree) on an external float distance triangle."""
     t = np.ascontiguousarray(tri, dtype=np.float32)
     out = np.zeros((2 * n - 1, 2), dtype=np.int32)
-    ref().ref_upgma_tree_from_distances(_p(t), n, int(modified), _p(out))
+    lib("ref").ref_upgma_tree_from_distances(_p(t), n, int(modified), _p(out))
     return out
 
 
@@ -251,7 +266,7 @@ class RefDp:
     """The reference's CProfile machinery behind oracle/ref_harness.cpp."""
 
     def __init__(self, n_seqs_for_rescale: int = 0, matrix_type: int = 2, pool_threads: int = 2):
-        self.lib = ref()
+        self.lib = lib("ref")
         self.h = C.c_void_p(self.lib.ref_dp_create(n_seqs_for_rescale, matrix_type, pool_threads))
 
     def close(self):
@@ -372,7 +387,7 @@ class RefSeqSet:
     """A set of CSequence objects inside the reference, built from residue letters."""
 
     def __init__(self, letters: list[str]):
-        self.lib = ref()
+        self.lib = lib("ref")
         arr = (C.c_char_p * len(letters))(*[s.encode("ascii") for s in letters])
         self.n = len(letters)
         self.h = C.c_void_p(self.lib.ref_seqset_create(arr, self.n))

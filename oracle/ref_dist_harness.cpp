@@ -1,6 +1,6 @@
 // oracle/ref_dist_harness.cpp -- C entry points over the UNMODIFIED reference's -dist_export path.
 //
-// TEST INFRASTRUCTURE ONLY.  Compiled by oracle/dist.mk together with the reference's own
+// TEST INFRASTRUCTURE ONLY.  Compiled by oracle/Makefile together with the reference's own
 // src/tree/DistanceCalculator.cpp into oracle/_ref/libfamsa_ref_dist.so, linked against
 // oracle/_ref/libfamsa_ref.so (the rest of the reference).  Nothing under famsa_b200/ may load it.
 //

@@ -1,6 +1,6 @@
 // oracle/ref_nj_harness.cpp -- C entry points over the UNMODIFIED reference's neighbour-joining guide tree (-gt nj).
 //
-// TEST INFRASTRUCTURE ONLY.  Compiled by oracle/nj.mk into oracle/_ref/libfamsa_ref_nj.so, linked against
+// TEST INFRASTRUCTURE ONLY.  Compiled by oracle/Makefile into oracle/_ref/libfamsa_ref_nj.so, linked against
 // oracle/_ref/libfamsa_ref.so, which already holds the reference's own src/tree/NeighborJoining.cpp.  Nothing under
 // famsa_b200/ may load it.
 //

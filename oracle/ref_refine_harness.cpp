@@ -1,6 +1,6 @@
 // oracle/ref_refine_harness.cpp -- the reference's refinement for the tests of famsa_prof_refine.  TEST INFRASTRUCTURE ONLY.
 //
-// Linked against _ref/libfamsa_ref.so (oracle/refine.mk), which holds the UNMODIFIED reference's CProfile
+// Linked against _ref/libfamsa_ref.so (oracle/Makefile), which holds the UNMODIFIED reference's CProfile
 // (src/core/profile.cpp: Condense, OptimizeGaps, CalculateCountersScores, CalculateTotalScore, Align) and CGappedSequence.
 // CFAMSA::RefineAlignment itself lives in src/msa_refinement.cpp, whose class drags in msa.cpp and the I/O libraries
 // (unbuildable here, DESIGN.md §2), so its loop (msa_refinement.cpp:7-66, 113-209) is restated below, line by line, on the

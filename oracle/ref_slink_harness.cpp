@@ -1,6 +1,6 @@
 // oracle/ref_slink_harness.cpp -- a C entry point over the UNMODIFIED reference's single-linkage guide tree (-gt slink).
 //
-// TEST INFRASTRUCTURE ONLY.  Compiled by oracle/slink.mk into oracle/_ref/libfamsa_ref_slink.so, linked against
+// TEST INFRASTRUCTURE ONLY.  Compiled by oracle/Makefile into oracle/_ref/libfamsa_ref_slink.so, linked against
 // oracle/_ref/libfamsa_ref.so, which already holds the reference's own src/tree/SingleLinkage.cpp.  Nothing under
 // famsa_b200/ may load it.
 //

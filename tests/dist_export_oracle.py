@@ -11,6 +11,8 @@ import math
 
 import numpy as np
 
+from oracle import pyoracle
+
 _INT64_MIN = np.int64(-2**63)
 
 
@@ -78,35 +80,16 @@ def csv_from_lcs(lcs_sq: np.ndarray, lens, ids, kind: int = 0, square: bool = Fa
 
 def lcs_square(codes, offsets, lens) -> np.ndarray:
     """n x n LCS lengths with the row as seq0, by the C restatement of the reference recurrence."""
-    from oracle import pyoracle
     n = len(lens)
     return pyoracle.lcs_rows(codes, offsets, lens, list(range(n)), n_col=n).astype(np.int64)
 
 
 # ---------------------------------------------------------------- the reference itself (oracle/_ref, where built)
-_REF_DIST = None
-
-
-def ref_dist_lib():
-    """oracle/_ref/libfamsa_ref_dist.so (oracle/dist.mk), or None where the reference was not built."""
-    global _REF_DIST
-    import ctypes as C
-    import os
-    path = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "libfamsa_ref_dist.so")
-    if _REF_DIST is None and os.path.exists(path):
-        lib = C.CDLL(path)
-        lib.ref_dist_export.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_int, C.c_int, C.c_int, C.c_char_p, C.c_int]
-        lib.ref_num2str_f32.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p]
-        lib.ref_num2str_f32.restype = C.c_uint64
-        _REF_DIST = lib
-    return _REF_DIST
-
-
 def ref_num2str(values) -> list[bytes]:
     """The reference's num2str on float32 values (one call for all of them)."""
     v = np.ascontiguousarray(values, dtype=np.float32)
     out = np.zeros(max(40 * v.size, 1), dtype=np.uint8)
-    n = ref_dist_lib().ref_num2str_f32(v.ctypes.data, v.size, out.ctypes.data)
+    n = pyoracle.lib("ref_dist").ref_num2str_f32(v.ctypes.data, v.size, out.ctypes.data)
     return out[:n].tobytes().split(b",")[:-1]
 
 
@@ -127,7 +110,7 @@ def ref_dist_export(letters, ids, kind: int = 0, square: bool = False, pid: bool
         fd, path = tempfile.mkstemp(suffix=".csv")
         os.close(fd)
     try:
-        rc = ref_dist_lib().ref_dist_export(la, ia, n, kind, int(square), int(pid), path.encode(), n_threads)
+        rc = pyoracle.lib("ref_dist").ref_dist_export(la, ia, n, kind, int(square), int(pid), path.encode(), n_threads)
         assert rc == 0
         if keep:
             return None

@@ -1,5 +1,5 @@
 """Generates the neighbour-joining (-gt nj) fixtures from the reference's own NeighborJoining<d>::run
-(oracle/_ref/libfamsa_ref_nj.so, built by oracle/nj.mk).  The reference ships no nj.dnd, so these trees are the goldens.
+(oracle/_ref/libfamsa_ref_nj.so, built by oracle/Makefile).  The reference ships no nj.dnd, so these trees are the goldens.
 
 Run where the reference's sources are at hand:  python tests/golden/make_nj.py
 Outputs (small, committed):

@@ -22,6 +22,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "..", ".."))
 sys.path.insert(0, os.path.join(HERE, ".."))
 from famsa_b200 import seqio  # noqa: E402
+from oracle import pyoracle  # noqa: E402
 
 REF = "/root/reference/test"
 OUT = os.path.join(HERE, "adeno_refined.npz")
@@ -51,7 +52,7 @@ def cases():
 def main():
     import refine_cases as rc
     import refine_oracle as ro
-    if not ro.have_ref():
+    if not pyoracle.have("ref_refine"):
         raise SystemExit("oracle/_ref/libfamsa_ref_refine.so is not built")
     out = {}
     for name, golden, leaves, seqs, merges in cases():

@@ -1,5 +1,5 @@
 """Generates the single-linkage (-gt slink) fixtures from the reference's test data and its own SingleLinkage<d>::run
-(oracle/_ref/libfamsa_ref_slink.so, built by oracle/slink.mk).
+(oracle/_ref/libfamsa_ref_slink.so, built by oracle/Makefile).
 
 Run where the reference's sources are at hand:  python tests/golden/make_slink.py [lrr]
 Outputs (small, committed):

@@ -3,6 +3,8 @@ and what the reference computes for them through oracle/_ref (RefDp: profile() o
 builds it, align(..., 1), the merged profile's rows in data order and its tables)."""
 from __future__ import annotations
 
+import os
+
 import numpy as np
 
 from famsa_b200 import seqio
@@ -143,3 +145,13 @@ def text_orientation(rows1: list[str], rows2: list[str]) -> bool:
         nz.append(int(np.count_nonzero(cnt[:-1])) + len(set(int(x) for x in last[last >= 0])))
     w1, w2 = len(rows1[0]) - 1, len(rows2[0]) - 1
     return not nz[0] * w2 < nz[1] * w1
+
+
+def host_mirror_input(path) -> None:
+    """The golden as the C++ mirror test (tests/cpp/test_host_profiles.cpp) reads it: gaps, score matrix, both inputs,
+    upgma.pp.fasta's rows."""
+    z = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "adeno_pp_rows.npz"))
+    lines = [" ".join(str(int(x)) for x in z["gaps"]), " ".join(str(int(x)) for x in z["score_matrix"].ravel())]
+    for key in ("rows1", "rows2", "gold_rows"):
+        lines += [str(len(z[key]))] + [str(r) for r in z[key]]
+    open(path, "w").write("\n".join(lines) + "\n")

@@ -3,51 +3,19 @@
 * numpy restatements of CProfile::CalculateTotalScore (profile.cpp:1368-1542, with its inclusion-exclusion table
   gap_ranges) and CProfile::OptimizeGaps (profile.cpp:436-689, with CGappedSequence::InsertGap / RemoveGap as string
   edits): the independent check of the device's k_ref_score_* and k_ref_optimize, which use other formulations;
-* the reference behind oracle/ref_refine_harness.cpp (oracle/_ref/libfamsa_ref_refine.so): its own CalculateTotalScore
-  and OptimizeGaps on given rows, and its progressive alignment followed by the restated RefineAlignment loop, with the
-  per-try trace and the final profile's tables; and its RefineAlignment loop on a given alignment;
+* the reference behind oracle/ref_refine_harness.cpp (oracle/_ref/libfamsa_ref_refine.so, opened by oracle/pyoracle.py):
+  its own CalculateTotalScore and OptimizeGaps on given rows, and its progressive alignment followed by the restated
+  RefineAlignment loop, with the per-try trace and the final profile's tables; and its RefineAlignment loop on a given
+  alignment;
 * total_score_rows: CalculateTotalScore vectorised, with a third formulation of the gap-open count, for widths the
   reference's (width+1)^2 / 2 tables and the restatement above cannot reach."""
 from __future__ import annotations
 
 import ctypes as C
-import os
 
 import numpy as np
 
-SO = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "oracle", "_ref", "libfamsa_ref_refine.so")
-_lib = None
-
-
-def have_ref() -> bool:
-    return os.path.exists(SO)
-
-
-def have_refine_rows() -> bool:
-    """The harness has rr_refine_rows (a library built where the reference's sources could not be read may be one
-    carried over from an older revision of ref_refine_harness.cpp, which has only the other entry points)."""
-    return have_ref() and hasattr(_load(), "rr_refine_rows")
-
-
-def _load():
-    global _lib
-    if _lib is None:
-        lib = C.CDLL(SO)
-        lib.rr_create.restype = C.c_void_p
-        lib.rr_create.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
-        lib.rr_destroy.argtypes = [C.c_void_p]
-        lib.rr_total_score.restype = C.c_int64
-        lib.rr_total_score.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
-        lib.rr_optimize_gaps.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_char_p]
-        lib.rr_align_refine.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_char_p,
-                                        C.c_char_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
-                                        C.c_void_p, C.c_void_p]
-        if hasattr(lib, "rr_refine_rows"):
-            lib.rr_refine_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_char_p,
-                                           C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
-                                           C.c_void_p, C.c_void_p]
-        _lib = lib
-    return _lib
+from oracle import pyoracle
 
 
 def _strs(xs):
@@ -59,7 +27,7 @@ class RefRefine:
     no_threads is what RefineAlignment passes to Align (> 1: the unbanded paths)."""
 
     def __init__(self, score_matrix, gaps, flags: int = 0, no_threads: int = 2):
-        self.lib = _load()
+        self.lib = pyoracle.lib("ref_refine")
         self.sm = np.ascontiguousarray(score_matrix, dtype=np.int64)
         self.g = np.ascontiguousarray(gaps, dtype=np.int64)
         self.h = C.c_void_p(self.lib.rr_create(self.sm.ctypes.data, self.g.ctypes.data, flags, no_threads))

@@ -1,14 +1,14 @@
-"""SingleLinkage<d>::run (-gt slink) for the tests: a verbatim restatement of the reference's pointer loops, and ctypes
-access to the reference's own run through oracle/_ref/libfamsa_ref_slink.so (oracle/ref_slink_harness.cpp)."""
+"""SingleLinkage<d>::run (-gt slink) for the tests: a verbatim restatement of the reference's pointer loops, and the
+reference's own run through oracle/_ref/libfamsa_ref_slink.so (oracle/ref_slink_harness.cpp, opened by
+oracle/pyoracle.py)."""
 from __future__ import annotations
 
 import ctypes as C
-import os
 
 import numpy as np
 
-_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_SLINK_SO = os.path.join(_ROOT, "oracle", "_ref", "libfamsa_ref_slink.so")
+from oracle import pyoracle
+
 DBL_MAX = float(np.finfo(np.float64).max)
 
 
@@ -52,7 +52,6 @@ def slink_restated(n: int, tri) -> list[tuple[int, int]]:
 
 def slink_distances(lcs_square: np.ndarray, lens, kind: int) -> np.ndarray:
     """The packed distance triangle SLINK reads: row i (the row, seq0) against j < i through Transform<double, kind>."""
-    from oracle import pyoracle
     n = len(lens)
     out = np.zeros(n * (n - 1) // 2, dtype=np.float64)
     at = 0
@@ -63,22 +62,11 @@ def slink_distances(lcs_square: np.ndarray, lens, kind: int) -> np.ndarray:
     return out
 
 
-_ref = None
-
-
-def have_ref() -> bool:
-    return os.path.exists(REF_SLINK_SO)
-
-
 def ref_slink_tree(letters: list[str], kind: int, n_threads: int = 8) -> np.ndarray:
     """The reference's own SingleLinkage<kind>::run on the set in this order: the n-1 merges, (n-1, 2) int32."""
-    global _ref
-    if _ref is None:
-        _ref = C.CDLL(REF_SLINK_SO)
-        _ref.ref_slink_tree.argtypes = [C.c_void_p, C.c_uint32, C.c_int, C.c_int, C.c_void_p]
     n = len(letters)
     arr = (C.c_char_p * max(n, 1))(*[s.encode("ascii") for s in letters])
     out = np.zeros((max(2 * n - 1, 1), 2), dtype=np.int32)
-    rc = _ref.ref_slink_tree(arr, n, kind, n_threads, out.ctypes.data_as(C.c_void_p))
+    rc = pyoracle.lib("ref_slink").ref_slink_tree(arr, n, kind, n_threads, out.ctypes.data_as(C.c_void_p))
     assert rc == 0
     return out[n:2 * n - 1] if n else out[:0]

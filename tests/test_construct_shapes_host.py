@@ -60,7 +60,8 @@ def test_fixture_matches_the_cases():
 def test_restated_walk_equals_the_reference(name):
     c = next(x for x in CASES if x["name"] == name)
     if S.crafted(c) and not pyoracle.have_ref_set_scores():
-        pytest.skip("the reference library predates ref_profile_set_scores (test_fixture_matches_the_cases covers the case)")
+        pytest.skip("oracle/_ref/libfamsa_ref.so has no ref_profile_set_scores "
+                    "(test_fixture_matches_the_cases covers the case)")
     t1, t2 = S.tables_of(c)
     ref = S.reference_merge(c)
     for mine, theirs in zip((t1, t2), ref["kids"]):

@@ -13,6 +13,7 @@ from famsa_b200 import seqio
 from famsa_b200.binding import WRITE_FN
 from conftest import GOLDEN, QUIRK_SEQS, random_set
 import dist_export_oracle as O
+from oracle import pyoracle
 from test_dist_export_host import MODES, TABLE, wrapping_floats
 
 pytestmark = pytest.mark.gpu
@@ -42,7 +43,7 @@ def test_adeno_goldens(engine, golden, name, square, pid, chunk_bytes):
 
 
 def expected(code_list, ids, kind, square, pid):
-    if O.ref_dist_lib() is not None:
+    if pyoracle.have("ref_dist"):
         letters = ["".join(LETTERS[c] for c in s) for s in code_list]
         return O.ref_dist_export(letters, ids, kind, square, pid, n_threads=8)
     codes, offsets, lens = seqio.pack(code_list)

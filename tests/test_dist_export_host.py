@@ -7,6 +7,7 @@ import pytest
 
 from conftest import GOLDEN
 import dist_export_oracle as O
+from oracle import pyoracle
 
 MODES = (("dist", False, False), ("pid", False, True), ("dist_sq", True, False), ("pid_sq", True, True))
 
@@ -69,7 +70,7 @@ def test_wrapping_floats():
     assert all(s == b"%d.000000" % x for s, x in zip(O.num2str(w), a.tolist()))
 
 
-needs_ref = pytest.mark.skipif(O.ref_dist_lib() is None, reason="oracle/_ref (the reference build) is not present")
+needs_ref = pytest.mark.skipif(not pyoracle.have("ref_dist"), reason="oracle/_ref/libfamsa_ref_dist.so not built")
 
 
 @needs_ref

@@ -13,7 +13,7 @@ import numpy as np
 import pytest
 
 import dp_shapes as D
-from conftest import ROOT
+from cpp_build import build_cpp
 from test_dp_shapes_gpu import LINE
 
 SMS = 132
@@ -27,10 +27,7 @@ FULL_LINE = re.compile(r"\[dp\] batch of \d+: class \d+ x \d+ \(first \d+ x \d+,
 
 @pytest.fixture(scope="module")
 def planner(tmp_path_factory):
-    exe = str(tmp_path_factory.mktemp("dp_plan") / "dp_plan_check")
-    subprocess.run(["g++", "-std=c++17", "-O1", "-Wall", "-Werror", os.path.join(ROOT, "tests", "cpp", "dp_plan_check.cpp"),
-                    "-o", exe], check=True)
-    return exe
+    return build_cpp("dp_plan_check", tmp_path_factory.mktemp("dp_plan"))
 
 
 def dims(jobs):

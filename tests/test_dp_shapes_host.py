@@ -196,7 +196,7 @@ def _gapped(rows) -> list[str]:
     return ["".join("-" if x < 0 else seqio.ALPHABET[x] for x in r) for r in np.concatenate([rows, last], axis=1)]
 
 
-@pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref is not built (the reference's sources are absent)")
+@pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref/libfamsa_ref.so not built")
 @pytest.mark.parametrize("card,wide", [(128, False), (300, False), (32768, False), (40000, False), (200, True)])
 def test_oracle_equals_reference_on_large_profiles(card, wide):
     """The reference's CProfile from the explicit gapped rows has the linear construction's tables, and its Align gives

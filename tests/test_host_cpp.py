@@ -1,27 +1,16 @@
 """Builds and runs the C++ host-mirror test (tests/cpp/test_host.cpp) against libfamsa_b200.so."""
-import os
 import subprocess
 
 import pytest
 
-from conftest import ROOT
-
-
-def build(tmp_path):
-    exe = str(tmp_path / "test_host")
-    cmd = ["g++", "-std=c++17", "-O1", os.path.join(ROOT, "tests", "cpp", "test_host.cpp"), "-o", exe,
-           "-L" + os.path.join(ROOT, "famsa_b200", "lib"), "-lfamsa_b200",
-           "-L" + os.path.join(ROOT, "oracle"), "-loracle",
-           "-Wl,-rpath," + os.path.join(ROOT, "famsa_b200", "lib"), "-Wl,-rpath," + os.path.join(ROOT, "oracle")]
-    subprocess.run(cmd, check=True)
-    return exe
+from cpp_build import build_cpp
 
 
 def test_host_mirror_compiles(tmp_path):
-    build(tmp_path)
+    build_cpp("test_host", tmp_path, famsa=True, oracle=True)
 
 
 @pytest.mark.gpu
 def test_host_mirror_runs(tmp_path):
-    out = subprocess.run([build(tmp_path)], capture_output=True, text=True)
+    out = subprocess.run([build_cpp("test_host", tmp_path, famsa=True, oracle=True)], capture_output=True, text=True)
     assert out.returncode == 0 and "host mirror ok" in out.stdout, out.stdout + out.stderr

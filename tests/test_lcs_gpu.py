@@ -231,7 +231,7 @@ def test_medoid_assignment_large(engine):
     assert np.isfinite(cost)
 
 
-@pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref not built")
+@pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref/libfamsa_ref.so not built")
 def test_medoid_assignment_sharded(engine):
     """famsa_lcs_assign_shard: three shards of one context, combined with an element-wise MIN (what the NCCL all-reduce
     does across GPUs), equal the unsharded famsa_lcs_assign bit for bit -- ragged lengths, unsorted input, a repeated seed."""
@@ -253,7 +253,7 @@ def test_medoid_assignment_sharded(engine):
         assert np.array_equal(a, want_a) and np.array_equal(d, want_d)
 
 
-@pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref not built")
+@pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref/libfamsa_ref.so not built")
 @pytest.mark.parametrize("modified", [False, True])
 def test_gpu_driven_upgma_tree(engine, modified):
     """Drop-in proof for HP-1: GPU LCS triangle -> host Transform<float, indel075_div_lcs> -> the reference's own,
@@ -382,7 +382,7 @@ def test_concurrent_callers_share_one_context(engine, adeno):
 from treeutil import prim_restated as _prim_restated  # noqa: E402
 
 
-@pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref not built")
+@pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref/libfamsa_ref.so not built")
 @pytest.mark.parametrize("case", ["family", "adeno", "quirky", "tiny"])
 def test_gpu_prim_tree(engine, adeno, case):
     """Drop-in proof for the DEFAULT guide tree (-gt sl): famsa_lcs_prim's MST edges, passed to the reference's own
@@ -440,7 +440,7 @@ def test_gpu_prim_golden_sl_tree(engine, monkeypatch, sequential):
     assert np.array_equal(ed, z["edge_dist"]) and np.array_equal(order, z["prim_order"])
 
 
-@pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref not built")
+@pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref/libfamsa_ref.so not built")
 def test_gpu_prim_lrr_golden_tree():
     """The reference's large default-guide-tree golden, test/LRR/sl.dnd (124 140 sequences; fixture lrr_sl.npz: the set in
     FAMSA's order and the CRC of the reference's MSTPrim tree, whose clades were checked against sl.dnd at generation).

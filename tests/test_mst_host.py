@@ -63,7 +63,7 @@ def test_kruskal_plus_replay_equals_sequential_prim(n, length, seed, kind):
         assert np.array_equal(g, w)
 
 
-@pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref not built")
+@pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref/libfamsa_ref.so not built")
 def test_replayed_mst_gives_the_reference_tree():
     codes, offsets, lens = seqio.synth_family(150, 80, seed=6)
     n = len(lens)

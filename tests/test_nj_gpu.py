@@ -30,12 +30,12 @@ from oracle import pyoracle as P
 import nj_oracle as N
 import upgma_cases as U
 from test_slink_gpu import live_sets
-from test_nj_host import build_cpp
+from cpp_build import build_cpp
 
 pytestmark = pytest.mark.gpu
 
 OK, E_INVALID, E_STATE = 0, 1, 4
-need_ref = pytest.mark.skipif(not N.have_ref(), reason="oracle/_ref not built")
+need_ref = pytest.mark.skipif(not P.have("ref_nj"), reason="oracle/_ref/libfamsa_ref_nj.so not built")
 
 
 def upload_letters(engine, letters):
@@ -182,7 +182,7 @@ def test_abi_contract():
 
 def test_host_mirror_nj_runs(engine, tmp_path):
     dump = tmp_path / "nj.txt"
-    r = subprocess.run([build_cpp(tmp_path), str(dump)], capture_output=True, text=True)
+    r = subprocess.run([build_cpp("test_host_nj", tmp_path, famsa=True), str(dump)], capture_output=True, text=True)
     assert r.returncode == 0 and "host mirror nj ok" in r.stdout, r.stdout + r.stderr
     lines = dump.read_text().split("\n")
     n = 200

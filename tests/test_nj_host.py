@@ -7,18 +7,18 @@ where the restatement reports what the reference turns into a cluster merged wit
 end with the restatement on the oracle's distances.  The adeno fixture is rebuilt by the restatement everywhere.
 Also compiles the C++ mirror's NeighborJoiningTree case."""
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
-from conftest import GOLDEN, ROOT, random_set
+from conftest import GOLDEN, random_set
 from famsa_b200 import seqio
 from oracle import pyoracle as P
 import nj_oracle as N
 import upgma_cases as U
+from cpp_build import build_cpp
 
-need_ref = pytest.mark.skipif(not N.have_ref(), reason="oracle/_ref not built")
+need_ref = pytest.mark.skipif(not P.have("ref_nj"), reason="oracle/_ref/libfamsa_ref_nj.so not built")
 FLT_MAX = np.float32(N.FLT_MAX)
 
 
@@ -123,14 +123,5 @@ def test_adeno_fixture_matches_restatement(kind):
     assert rc == 0 and np.array_equal(z[f"tree{kind}"], want)
 
 
-def build_cpp(tmp_path):
-    exe = str(tmp_path / "test_host_nj")
-    cmd = ["g++", "-std=c++17", "-O1", "-Wall", os.path.join(ROOT, "tests", "cpp", "test_host_nj.cpp"), "-o", exe,
-           "-L" + os.path.join(ROOT, "famsa_b200", "lib"), "-lfamsa_b200",
-           "-Wl,-rpath," + os.path.join(ROOT, "famsa_b200", "lib")]
-    subprocess.run(cmd, check=True)
-    return exe
-
-
 def test_host_mirror_nj_compiles(tmp_path):
-    build_cpp(tmp_path)
+    build_cpp("test_host_nj", tmp_path, famsa=True)

@@ -10,7 +10,7 @@ from dp_cases import check_against_reference, random_tree, reference_merges
 from famsa_b200 import seqio
 from oracle import pyoracle
 
-needs_ref = pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref not built")
+needs_ref = pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref/libfamsa_ref.so not built")
 
 
 def test_oracle_pp_golden():

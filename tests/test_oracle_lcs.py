@@ -45,7 +45,7 @@ def test_oracle_distance_golden(adeno):
             assert abs(d - adeno["dist"][i, j]) < 1e-6 * max(1.0, abs(d)) + 6e-7
 
 
-needs_ref = pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref not built")
+needs_ref = pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref/libfamsa_ref.so not built")
 
 
 @needs_ref

@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 
 import profile_mode_cases as pmc
+from cpp_build import build_cpp
 import refine_cases as rc
 import refine_oracle as ro
 import refine_shapes as S
@@ -20,7 +21,7 @@ from famsa_b200.binding import FamsaError
 from oracle import pyoracle
 
 pytestmark = pytest.mark.gpu
-need_ref = pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref (the compiled reference) is not built")
+need_ref = pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref/libfamsa_ref.so not built")
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
@@ -225,7 +226,8 @@ def refine_root_case():
     return next(c for c in S.refine_cases() if c["name"] == "ids_not_padded")
 
 
-@pytest.mark.skipif(not ro.have_refine_rows(), reason="oracle/_ref/libfamsa_ref_refine.so with rr_refine_rows not built")
+@pytest.mark.skipif(not pyoracle.have("ref_refine", "rr_refine_rows"),
+                    reason="oracle/_ref/libfamsa_ref_refine.so not built, or built without rr_refine_rows")
 def test_refine_root_and_refine_state(eng):
     """A user's alignment as a refine root: famsa_prof_put_rows -> famsa_prof_refine is RefineAlignment of those rows.  A
     later famsa_prof_put_rows leaves famsa_prof_refined_rows alone."""
@@ -255,8 +257,7 @@ def test_refine_root_and_refine_state(eng):
 def test_host_mirror_runs(tmp_path):
     """famsa_b200::AlignProfiles reproduces upgma.pp.fasta through FinalizeGaps' runs and the output order."""
     import subprocess
-    from test_profile_mode_host import build_host_mirror, host_mirror_input
-    exe = build_host_mirror(tmp_path)
-    host_mirror_input(tmp_path / "pp.txt")
+    exe = build_cpp("test_host_profiles", tmp_path, famsa=True)
+    pmc.host_mirror_input(tmp_path / "pp.txt")
     out = subprocess.run([exe, str(tmp_path / "pp.txt")], capture_output=True, text=True)
     assert out.returncode == 0 and "host mirror profiles ok" in out.stdout, out.stdout + out.stderr

@@ -10,8 +10,9 @@ from conftest import ROOT
 from famsa_b200 import profiles, seqio
 from oracle import pyoracle
 import profile_mode_cases as pmc
+from cpp_build import build_cpp
 
-need_ref = pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref (the compiled reference) is not built")
+need_ref = pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref/libfamsa_ref.so not built")
 
 
 def test_encode_gapped():
@@ -121,25 +122,6 @@ def test_golden_fixture_rule():
     assert np.array_equal(z["path"], pp["path"]) and int(z["total"]) == int(pp["total"])
 
 
-def build_host_mirror(tmp_path) -> str:
-    """tests/cpp/test_host_profiles.cpp against libfamsa_b200.so (no GPU needed to build it)."""
-    import subprocess
-    exe = str(tmp_path / "test_host_profiles")
-    lib = os.path.join(ROOT, "famsa_b200", "lib")
-    subprocess.run(["g++", "-std=c++17", "-O1", "-Wall", "-Werror", os.path.join(ROOT, "tests", "cpp", "test_host_profiles.cpp"),
-                    "-o", exe, "-L" + lib, "-lfamsa_b200", "-Wl,-rpath," + lib], check=True)
-    return exe
-
-
-def host_mirror_input(path) -> None:
-    """The golden as the C++ mirror test reads it: gaps, score matrix, both inputs, upgma.pp.fasta's rows."""
-    z = np.load(os.path.join(ROOT, "tests", "golden", "adeno_pp_rows.npz"))
-    lines = [" ".join(str(int(x)) for x in z["gaps"]), " ".join(str(int(x)) for x in z["score_matrix"].ravel())]
-    for key in ("rows1", "rows2", "gold_rows"):
-        lines += [str(len(z[key]))] + [str(r) for r in z[key]]
-    open(path, "w").write("\n".join(lines) + "\n")
-
-
 def test_host_mirror_compiles(tmp_path):
-    build_host_mirror(tmp_path)
-    host_mirror_input(tmp_path / "pp.txt")
+    build_cpp("test_host_profiles", tmp_path, famsa=True)
+    pmc.host_mirror_input(tmp_path / "pp.txt")

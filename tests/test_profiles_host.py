@@ -5,7 +5,7 @@ import pytest
 from famsa_b200 import profiles, seqio
 from oracle import pyoracle
 
-needs_ref = pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref not built")
+needs_ref = pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref/libfamsa_ref.so not built")
 
 
 @needs_ref

@@ -9,9 +9,10 @@ import dp_cases
 import refine_cases as rc
 import refine_oracle
 from famsa_b200.binding import REFINE_NO_GAP_OPT, REFINE_NO_TOTAL_SCORE, FamsaError
+from oracle import pyoracle
 
 pytestmark = [pytest.mark.gpu,
-              pytest.mark.skipif(not refine_oracle.have_ref(), reason="oracle/_ref/libfamsa_ref_refine.so not built")]
+              pytest.mark.skipif(not pyoracle.have("ref_refine"), reason="oracle/_ref/libfamsa_ref_refine.so not built")]
 
 
 @pytest.fixture(scope="module")

@@ -12,8 +12,9 @@ import dp_cases
 import refine_cases as rc
 import refine_oracle as ro
 from famsa_b200 import profiles
+from oracle import pyoracle
 
-need_ref = pytest.mark.skipif(not ro.have_ref(), reason="oracle/_ref/libfamsa_ref_refine.so not built")
+need_ref = pytest.mark.skipif(not pyoracle.have("ref_refine"), reason="oracle/_ref/libfamsa_ref_refine.so not built")
 GAP = ro.GAP
 
 
@@ -89,7 +90,7 @@ def test_total_score_rows_equals_restatement_and_reference(kind, seed):
     cn = counters(a, sm, g)
     got = ro.total_score_rows(a, cn, sm, g)
     assert got == ro.total_score(a, cn, sm, g)
-    if ro.have_ref() and kind != "no_len1":
+    if pyoracle.have("ref_refine") and kind != "no_len1":
         ref = ro.RefRefine(sm, g)
         assert got == ref.total_score([rc.to_letters(r) for r in a])
         ref.close()
@@ -171,7 +172,8 @@ def test_trace_matches_counts(n, flags):
     assert c["n_realigned"] == 100 or c["n_tries"] == 2000
 
 
-@pytest.mark.skipif(not ro.have_refine_rows(), reason="the harness library has no rr_refine_rows: rebuild oracle/refine.mk")
+@pytest.mark.skipif(not pyoracle.have("ref_refine", "rr_refine_rows"),
+                    reason="oracle/_ref/libfamsa_ref_refine.so not built, or built without rr_refine_rows")
 def test_refine_rows_is_the_loop_of_align_refine():
     """rr_refine_rows on the unrefined rows of rr_align_refine gives the same refinement, try for try."""
     n = 30

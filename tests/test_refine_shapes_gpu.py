@@ -23,9 +23,11 @@ import refine_cases as rc
 import refine_oracle as ro
 import refine_shapes as S
 from famsa_b200.binding import REFINE_NO_TOTAL_SCORE, FamsaError
+from oracle import pyoracle
 
 pytestmark = pytest.mark.gpu
-need_ref = pytest.mark.skipif(not ro.have_refine_rows(), reason="oracle/_ref/libfamsa_ref_refine.so with rr_refine_rows not built")
+need_ref = pytest.mark.skipif(not pyoracle.have("ref_refine", "rr_refine_rows"),
+                              reason="oracle/_ref/libfamsa_ref_refine.so not built, or built without rr_refine_rows")
 HERE = os.path.dirname(os.path.abspath(__file__))
 SCORE = {c["name"]: c for c in S.score_cases()}
 REFINE = {c["name"]: c for c in S.refine_cases()}
@@ -92,7 +94,7 @@ def test_score(eng, name):
     assert width == w and np.array_equal(out, a), "n_refinements = 0 must return the rows unchanged"
     want = ro.total_score_rows(a, S.tables(a, sm, g)[1], sm, g)
     assert total == want
-    if w <= 4096 and ro.have_ref():
+    if w <= 4096 and pyoracle.have("ref_refine"):
         ref = ro.RefRefine(sm, g)
         assert total == ref.total_score([rc.to_letters(r) for r in a])
         ref.close()

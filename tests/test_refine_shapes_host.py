@@ -12,10 +12,11 @@ import dp_shapes
 import refine_cases as rc
 import refine_oracle as ro
 import refine_shapes as S
+from oracle import pyoracle
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SRC = open(os.path.join(ROOT, "famsa_b200", "csrc", "refine.cu")).read()
-need_ref = pytest.mark.skipif(not ro.have_ref(), reason="oracle/_ref/libfamsa_ref_refine.so not built")
+need_ref = pytest.mark.skipif(not pyoracle.have("ref_refine"), reason="oracle/_ref/libfamsa_ref_refine.so not built")
 
 
 def test_constants_match_refine_cu():

@@ -167,7 +167,7 @@ def _tree_worker(rank, world, port, n, out_dir):
     dist.destroy_process_group()
 
 
-@pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref not built")
+@pytest.mark.skipif(not pyoracle.have_ref(), reason="oracle/_ref/libfamsa_ref.so not built")
 @pytest.mark.parametrize("world", [2, 3])
 def test_subtree_sharded_resident_alignment(tmp_path, world):
     """HP-2 on several ranks with resident profiles: whole subtrees per rank (no communication), subtree roots handed

@@ -13,13 +13,14 @@ import pytest
 import famsa_b200
 from famsa_b200 import seqio
 from conftest import GOLDEN, random_set
+from oracle import pyoracle
 import slink_oracle as S
-from test_slink_host import build_cpp
+from cpp_build import build_cpp
 
 pytestmark = pytest.mark.gpu
 
 OK, E_INVALID, E_STATE = 0, 1, 4
-need_ref = pytest.mark.skipif(not S.have_ref(), reason="oracle/_ref not built")
+need_ref = pytest.mark.skipif(not pyoracle.have("ref_slink"), reason="oracle/_ref/libfamsa_ref_slink.so not built")
 
 
 def engine_kinds(monkeypatch, sequential):
@@ -179,7 +180,7 @@ def test_abi_contract():
 
 def test_host_mirror_slink_runs(engine, tmp_path):
     dump = tmp_path / "slink.txt"
-    r = subprocess.run([build_cpp(tmp_path), str(dump)], capture_output=True, text=True)
+    r = subprocess.run([build_cpp("test_host_slink", tmp_path, famsa=True), str(dump)], capture_output=True, text=True)
     assert r.returncode == 0 and "host mirror slink ok" in r.stdout, r.stdout + r.stderr
     lines = dump.read_text().split("\n")
     n = 200

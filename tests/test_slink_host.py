@@ -4,15 +4,15 @@ of each side.  Checked against a verbatim restatement of the reference's pointer
 random triangles full of ties, and on the committed adeno fixture from its LCS values alone.  Also compiles the C++
 mirror's SingleLinkageTree case."""
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
-from conftest import GOLDEN, ROOT
+from conftest import GOLDEN
 from famsa_b200 import mst, seqio
 from oracle import pyoracle
 import slink_oracle as S
+from cpp_build import build_cpp
 
 NEVER = float(np.nextafter(S.DBL_MAX, 0.0))      # Transform's distance for LCS 0
 
@@ -81,14 +81,5 @@ def test_adeno_fixture_from_golden_lcs(kind):
         assert [tuple(int(x) for x in r) for r in z["tree"]] == want
 
 
-def build_cpp(tmp_path):
-    exe = str(tmp_path / "test_host_slink")
-    cmd = ["g++", "-std=c++17", "-O1", "-Wall", os.path.join(ROOT, "tests", "cpp", "test_host_slink.cpp"), "-o", exe,
-           "-L" + os.path.join(ROOT, "famsa_b200", "lib"), "-lfamsa_b200",
-           "-Wl,-rpath," + os.path.join(ROOT, "famsa_b200", "lib")]
-    subprocess.run(cmd, check=True)
-    return exe
-
-
 def test_host_mirror_slink_compiles(tmp_path):
-    build_cpp(tmp_path)
+    build_cpp("test_host_slink", tmp_path, famsa=True)

@@ -173,7 +173,7 @@ def test_vectorised_prim_equals_kruskal_replay():
             assert np.array_equal(g, w)
 
 
-@pytest.mark.skipif(not P.have_ref(), reason="oracle/_ref not built")
+@pytest.mark.skipif(not P.have_ref(), reason="oracle/_ref/libfamsa_ref.so not built")
 @pytest.mark.parametrize("case", ["family", "abc3", "carry_sorted", "carry_shuffled"])
 def test_vectorised_prim_gives_reference_tree(case):
     codes, offsets, lens, exact = host_sets()[case]

@@ -10,7 +10,8 @@ import subprocess
 import numpy as np
 import pytest
 
-from conftest import GOLDEN, ROOT
+from conftest import GOLDEN
+from cpp_build import build_cpp
 from dp_cases import random_tree
 from famsa_b200.schedule import ready_levels
 
@@ -23,9 +24,7 @@ TREES = [("adeno_slink_tree", "tree"), ("adeno_nj_tree", "tree0"), ("adeno_nj_tr
 
 @pytest.fixture(scope="module")
 def check(tmp_path_factory):
-    exe = str(tmp_path_factory.mktemp("tree_plan") / "tree_plan_check")
-    subprocess.run(["g++", "-std=c++17", "-O1", "-Wall", "-Werror", os.path.join(ROOT, "tests", "cpp", "tree_plan_check.cpp"),
-                    "-o", exe], check=True)
+    exe = build_cpp("tree_plan_check", tmp_path_factory.mktemp("tree_plan"))
 
     def run(*args, stdin="", fused=None):
         env = {k: v for k, v in os.environ.items() if k != "FAMSA_PROF_FUSED"}

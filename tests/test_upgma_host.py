@@ -9,7 +9,7 @@ from famsa_b200 import seqio
 from oracle import pyoracle as P
 import upgma_cases as U
 
-need_ref = pytest.mark.skipif(not P.have_ref(), reason="oracle/_ref not built")
+need_ref = pytest.mark.skipif(not P.have_ref(), reason="oracle/_ref/libfamsa_ref.so not built")
 NEVER = np.float32(np.nextafter(np.float64(np.finfo(np.float32).max), 0.0))     # Transform of LCS 0
 
 

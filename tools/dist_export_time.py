@@ -22,6 +22,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import famsa_b200  # noqa: E402
 from famsa_b200 import seqio  # noqa: E402
+from oracle import pyoracle  # noqa: E402
 import dist_export_oracle as O  # noqa: E402
 
 LETTERS = "ARNDCQEGHILKMFPSTWYVBZX*"
@@ -64,7 +65,7 @@ def main():
     eng = famsa_b200.Engine(0)
     eng.upload(codes, offsets, lens)
     eng.dist_export(ids[:], pid=True, out=Discard())            # warm-up: allocations, pinned buffers
-    have_ref = O.ref_dist_lib() is not None
+    have_ref = pyoracle.have("ref_dist")
     letters = ["".join(LETTERS[c] for c in codes[offsets[i]:offsets[i] + lens[i]]) for i in range(a.n)] if have_ref else None
     with tempfile.TemporaryDirectory() as tmp:
         for mode, square, pid in MODES:

@@ -23,6 +23,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import famsa_b200  # noqa: E402
 from famsa_b200 import seqio  # noqa: E402
+from oracle import pyoracle  # noqa: E402
 import nj_oracle as N  # noqa: E402
 
 SETS = (("2k", 2000, 400, 1), ("C2", 10000, 400, 1))
@@ -67,7 +68,7 @@ def main():
         finally:
             eng.close()
         rec = dict(set=label, n=n, len=length, gpu=name, power_limit=power, device=dev)
-        if N.have_ref() and n <= a.ref_max:
+        if pyoracle.have("ref_nj") and n <= a.ref_max:
             letters = [seqio.decode(codes[int(o):int(o) + int(ln)]) for o, ln in zip(offsets, lens)]
             want, sec = N.ref_tree(letters, 0)
             rec.update(ref_threads=1, ref_wall_s=round(sec, 3), same_as_ref=bool(np.array_equal(tree, want)))

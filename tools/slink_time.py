@@ -23,6 +23,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import famsa_b200  # noqa: E402
 from famsa_b200 import seqio  # noqa: E402
+from oracle import pyoracle  # noqa: E402
 import slink_oracle as S  # noqa: E402
 
 SETS = (("C2", 10000, 400, 1), ("40k", 40000, 60, 45))
@@ -73,7 +74,7 @@ def main():
             eng.close()
         rec = dict(set=label, n=n, len=length, gpu=name, power_limit=power, boruvka=boruvka, sequential=sequential,
                    engines_agree=bool(np.array_equal(tree, tree_seq)))
-        if S.have_ref() and not a.no_ref:
+        if pyoracle.have("ref_slink") and not a.no_ref:
             letters = [seqio.decode(codes[int(o):int(o) + int(ln)]) for o, ln in zip(offsets, lens)]
             t0 = time.perf_counter()
             want = S.ref_slink_tree(letters, 0, n_threads=threads)
