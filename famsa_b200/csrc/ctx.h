@@ -78,13 +78,13 @@ struct LcsState {
     DevBuf d_lcs_tri;                        // resident LCS triangle (prim, UPGMA, export), elem_bytes() wide
     DevBuf d_dist_tri;                       // distance triangle: float64 for the Boruvka rounds, float32 for UPGMA and NJ
     DevBuf d_nj_half;                        // NJ's compaction target: the float triangle of n/2 + 1 rows
-    DevBuf d_side_idx, d_side_rows;          // lcs_side_rows: row of a flagged sequence in d_side_rows or -1; its u32 rows
+    DevBuf d_side_idx, d_side_rows;          // lcs_side_rows: a sequence's row in d_side_rows or -1; those u32 rows
     DevBuf d_tree_state, d_tree_out, d_tree_cand;   // k_prim's or k_upgma's state, outputs and block candidates
     DevBuf d_mst_comp, d_mst_best, d_mst_part;      // Boruvka rounds
     // per-call scratch
     DevBuf d_tiles, d_res, d_refpos, d_ids_a, d_ids_b, d_out_stage, d_masks64, d_exact_rows, d_x64;
     // famsa_dist_export: per-sequence tables, the two device text chunks and their pinned host twins
-    DevBuf d_dx_meta, d_dx_ids, d_dx_colq, d_dx_chunk[2];
+    DevBuf d_dx_meta, d_dx_ids, d_dx_chunk[2];
     char* h_dx_chunk[2] = {nullptr, nullptr};
     size_t h_dx_chunk_cap = 0;
     cudaEvent_t ev_dx[6] = {};               // per chunk buffer: format start, format end, copy done
@@ -276,8 +276,6 @@ int lcs_rows(famsa_ctx* ctx, const uint32_t* h_ref_ids, uint32_t n_ref, const ui
              int elem_bytes, cudaStream_t stream, uint32_t g_begin = 0, uint32_t g_end = 0xffffffffu);
 int lcs_side_rows(famsa_ctx* ctx, cudaStream_t st);
 int lcs_pow075_f64(famsa_ctx* ctx, cudaStream_t st);
-int lcs_exact_block(famsa_ctx* ctx, const std::vector<uint32_t>& rows, const uint32_t* d_col_ids, uint32_t n_col, void* d_out,
-                    int elem_bytes, cudaStream_t st);
 // tree.cu
 int lcs_upgma(famsa_ctx* ctx, int kind, int modified, int32_t* h_tree, const void* d_tri_in = nullptr, int tri_eb = 2);
 int lcs_nj(famsa_ctx* ctx, int kind, int32_t* h_tree);

@@ -4,11 +4,10 @@
 // Transform of its worker threads and the single-threaded gather loop that prints every value with
 // NumericConversions::Double2PChar (src/utils/conversion.h:52-119).  See DESIGN.md section 3.
 //
-//   * LCS: the packed triangle of the caller's order, computed once by the tile kernel and kept in HBM (row = seq0, the
-//     dropped-carry rows already recomputed by the exact path).  Square mode reads the upper part from the mirror
-//     cell, which is only right when neither sequence is orientation dependent: rows of flagged sequences come from
-//     side rows (lcs_side_rows), columns of flagged sequences from an exact block (every row as seq0 against them), and
-//     the diagonal of the others is the number of residues that can match (codes < 20).
+//   * LCS: the packed triangle of the caller's order, computed once by the tile kernel and kept in HBM.  Triangle mode
+//     reads it with row = seq0 (the dropped-carry rows recomputed by the exact path).  Square mode reads what k_prim
+//     reads, through lcs_seq0: the true-LCS triangle and the side rows (lcs_side_rows) of the sequences whose value
+//     depends on being seq0; the diagonal of the others is the number of residues that can match (codes < 20).
 //   * Text: pass 1 sums every row's byte count (the width of a value depends on it alone); the host cuts the rows into
 //     chunks and prefix-sums the row offsets; pass 2, one block per row, formats 1024 values at a time: per-value
 //     lengths, a block scan, the characters into shared memory at the destination's 16-byte phase, then aligned 16-byte
@@ -33,17 +32,11 @@ constexpr int kMaxValueChars = 40;                                // "9223372036
 constexpr uint64_t kDefaultChunk = 32ull << 20;
 
 struct DistParams {
-    const void* tri;               // packed LCS triangle, caller order, row = seq0
-    int eb;                        // its element bytes
-    uint32_t n;
+    Seq0View lcs;                  // square; triangle: tri is the packed triangle with row = seq0, no side rows
     const uint32_t* lens;          // caller order
     const double* pow075;          // (double) pow(i, 0.75), host libm
     int kind, pid, square;
-    const int* side_idx;           // square: row of a flagged sequence in `side` / column in `colq`, else -1
-    const uint32_t* side;          // nq x n: flagged sequence as seq0 against every column
-    const uint32_t* colq;          // n x nq: every sequence as seq0 against the flagged ones
-    uint32_t nq;
-    const uint32_t* diag;          // square: LCS of a sequence with itself (unflagged ones)
+    const uint32_t* diag;          // square: LCS of a sequence with itself (those without a side row)
     const char* ids;
     const unsigned long long* id_off;   // n + 1
 };
@@ -103,24 +96,15 @@ __device__ __forceinline__ void put_value(char* dst, unsigned long long a, unsig
 // cells
 // ------------------------------------------------------------------------------------------------
 
-__device__ __forceinline__ uint32_t tri_at(const DistParams& P, uint32_t i, uint32_t j)          // i > j
-{
-    return lcs_load(P.tri, P.eb, tri_index(i, j));
-}
-
 // LCS with r as seq0 and c streamed (c < r in triangle mode)
 __device__ __forceinline__ uint32_t cell_lcs(const DistParams& P, uint32_t r, uint32_t c)
 {
     if (P.square) {
-        const int sr = P.side_idx[r];
-        if (sr >= 0) return P.side[(size_t)sr * P.n + c];
-        if (c == r) return P.diag[r];
-        if (c > r) {
-            const int sc = P.side_idx[c];
-            return sc >= 0 ? P.colq[(size_t)r * P.nq + sc] : tri_at(P, c, r);
-        }
+        const int s = side_row<true>(P.lcs, r);
+        if (c == r && s < 0) return P.diag[r];
+        if (c > r || s >= 0) return lcs_seq0(P.lcs, s, r, c);
     }
-    return tri_at(P, r, c);
+    return lcs_load(P.lcs.tri, P.lcs.eb, tri_index(r, c));      // lcs_seq0's cell for c < r without a side row
 }
 
 __device__ __forceinline__ float cell_value(const DistParams& P, uint32_t r, uint32_t c)
@@ -153,7 +137,7 @@ __global__ void __launch_bounds__(kFmtThreads) k_dist_row_bytes(const DistParams
     using Reduce = cub::BlockReduce<unsigned long long, kFmtThreads>;
     __shared__ typename Reduce::TempStorage tmp;
     const uint32_t r = blockIdx.x;
-    const uint32_t ncol = P.square ? P.n : r;
+    const uint32_t ncol = P.square ? P.lcs.n : r;
     unsigned long long sum = 0;
     for (uint32_t c = threadIdx.x; c < ncol; c += kFmtThreads) {
         unsigned long long a, b;
@@ -164,8 +148,9 @@ __global__ void __launch_bounds__(kFmtThreads) k_dist_row_bytes(const DistParams
     if (threadIdx.x == 0) row_bytes[r] = sum + (P.id_off[r + 1] - P.id_off[r]) + 1;
 }
 
-// pass 2: rows [r0, r0 + gridDim.x) into `out`, row r at row_start[r] - row_start[r0]
-__global__ void __launch_bounds__(kFmtThreads) k_dist_format(const DistParams P, uint32_t r0,
+// pass 2: rows [r0, r0 + gridDim.x) into `out`, row r at row_start[r] - row_start[r0].  Five blocks per SM: what the
+// stage's shared memory allows, and 48 registers hold a thread's four cells without spilling.
+__global__ void __launch_bounds__(kFmtThreads, 5) k_dist_format(const DistParams P, uint32_t r0,
                                                              const unsigned long long* __restrict__ row_start,
                                                              char* __restrict__ out)
 {
@@ -174,7 +159,7 @@ __global__ void __launch_bounds__(kFmtThreads) k_dist_format(const DistParams P,
     __shared__ __align__(16) char stage[kFmtTile * kMaxValueChars + 32];
     __shared__ uint32_t tile_total;
     const uint32_t r = r0 + blockIdx.x;
-    const uint32_t ncol = P.square ? P.n : r;
+    const uint32_t ncol = P.square ? P.lcs.n : r;
     char* row = out + (row_start[r] - row_start[r0]);
 
     const uint64_t id0 = P.id_off[r], idlen = P.id_off[r + 1] - id0;
@@ -263,11 +248,11 @@ int dist_export(famsa_ctx* ctx, int kind, int square, int pid, const char* ids, 
     if (!S.ev_dx[0])
         for (int e = 0; e < 6; ++e) FB_CUDA(cudaEventCreateWithFlags(&S.ev_dx[e], e % 3 == 2 ? cudaEventDisableTiming : cudaEventDefault));
 
-    // 1. the LCS triangle in caller order (row = seq0), resident for the whole call
+    // 1. the LCS triangle in caller order, resident for the whole call: row = seq0 (triangle), the true LCS (square)
     if (S.d_lcs_tri.reserve(std::max<uint64_t>(pairs, 1) * eb)) return nomem(ctx, "the LCS triangle", pairs * eb);
     S.tiles_marked = false;
     FB_CUDA(cudaEventRecord(ctx->ev[0], st));
-    FB_TRY(lcs_triangle(ctx, 0, n, S.d_lcs_tri.p, eb, st));
+    FB_TRY(lcs_triangle(ctx, 0, n, S.d_lcs_tri.p, eb, st, nullptr, 1, nullptr, /*quirk_fixups=*/!square));
     FB_CUDA(cudaEventRecord(ctx->ev[3], st));
     FB_CUDA(cudaStreamSynchronize(st));
     float lcs_total = 0.f, lcs_main = 0.f;
@@ -288,8 +273,7 @@ int dist_export(famsa_ctx* ctx, int kind, int square, int pid, const char* ids, 
     if (id_bytes) FB_CUDA(cudaMemcpyAsync(S.d_dx_ids.p, ids + id_offsets[0], id_bytes, cudaMemcpyHostToDevice, st));
     FB_CUDA(cudaMemcpyAsync(d_id_off, id_off.data(), sizeof(unsigned long long) * (n + 1), cudaMemcpyHostToDevice, st));
 
-    // square: rows of the flagged sequences (seq0 = the flagged one) and their columns (seq0 = every other sequence)
-    const uint32_t nq = square ? (uint32_t)S.h_quirky.size() : 0;
+    // square: the diagonal and the side rows
     FB_CUDA(cudaEventRecord(ctx->ev_host[0], st));
     if (square) {
         k_dist_diag<<<(n + 7) / 8, 256, 0, st>>>(S.d_raw_codes.as<int8_t>(), S.d_raw_off.as<uint64_t>(), S.d_raw_len.as<uint32_t>(), n, d_diag);
@@ -297,22 +281,13 @@ int dist_export(famsa_ctx* ctx, int kind, int square, int pid, const char* ids, 
         ctx->launches++;
         FB_TRY(lcs_side_rows(ctx, st));
     }
-    if (nq) {
-        if (S.d_dx_colq.reserve(sizeof(uint32_t) * nq * (size_t)n)) return nomem(ctx, "the flagged columns", sizeof(uint32_t) * nq * (uint64_t)n);
-        FB_TRY(S.d_ids_a.reserve(sizeof(uint32_t) * nq));
-        FB_CUDA(cudaMemcpyAsync(S.d_ids_a.p, S.h_quirky.data(), sizeof(uint32_t) * nq, cudaMemcpyHostToDevice, st));
-        std::vector<uint32_t> all(n);
-        for (uint32_t r = 0; r < n; ++r) all[r] = r;
-        FB_TRY(lcs_exact_block(ctx, all, S.d_ids_a.as<uint32_t>(), nq, S.d_dx_colq.p, 4, st));
-    }
     if (!pid) FB_TRY(lcs_pow075_f64(ctx, st));
 
     DistParams P{};
-    P.tri = S.d_lcs_tri.p; P.eb = eb; P.n = n;
+    P.lcs = Seq0View{S.d_lcs_tri.p, eb, n, S.d_side_idx.as<int>(), S.d_side_rows.as<uint32_t>()};
     P.lens = S.d_raw_len.as<uint32_t>();
     P.pow075 = S.d_pow075_f64.as<double>();
     P.kind = kind; P.pid = pid; P.square = square;
-    P.side_idx = S.d_side_idx.as<int>(); P.side = S.d_side_rows.as<uint32_t>(); P.colq = S.d_dx_colq.as<uint32_t>(); P.nq = nq;
     P.diag = d_diag;
     P.ids = S.d_dx_ids.as<char>(); P.id_off = d_id_off;
 

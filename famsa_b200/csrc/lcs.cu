@@ -697,6 +697,42 @@ static int mark_tiles_begin(famsa_ctx* ctx, cudaStream_t st)
     return FAMSA_OK;
 }
 
+// The tiles of one call, per piece and limb-count class (index NL).  upload() copies all of them into d_tiles in one
+// go, piece after piece and class after class, and marks the start of the tile span; launch(b), called for the pieces
+// in order, issues piece b's classes in ascending NL on the given stream.
+struct TilePlan {
+    std::vector<std::vector<std::vector<uint3>>> lists;
+    size_t total = 0, at = 0;
+    explicit TilePlan(int n_pieces) : lists(n_pieces, std::vector<std::vector<uint3>>(kMaxNL + 1)) {}
+    // mask group g against the streamed items [0, q_end), kTileQ per tile
+    void add(int b, uint32_t g, uint32_t nl, uint32_t q_end)
+    {
+        for (uint32_t q0 = 0; q0 < q_end; q0 += kTileQ, ++total)
+            lists[b][nl].push_back(make_uint3(g, q0, std::min(q_end, q0 + (uint32_t)kTileQ)));
+    }
+    int upload(famsa_ctx* ctx, cudaStream_t st) const
+    {
+        std::vector<uint3> flat;
+        flat.reserve(total);
+        for (auto& piece : lists)
+            for (auto& v : piece) flat.insert(flat.end(), v.begin(), v.end());
+        FB_TRY(ctx->lcs.d_tiles.reserve(sizeof(uint3) * std::max<size_t>(total, 1)));
+        if (total) FB_CUDA(cudaMemcpyAsync(ctx->lcs.d_tiles.p, flat.data(), sizeof(uint3) * total, cudaMemcpyHostToDevice, st));
+        return mark_tiles_begin(ctx, st);
+    }
+    int launch(famsa_ctx* ctx, int b, TileParams P, cudaStream_t st)
+    {
+        for (uint32_t nl = 1; nl <= (uint32_t)kMaxNL; ++nl) {
+            const auto& v = lists[b][nl];
+            if (v.empty()) continue;
+            P.tiles = ctx->lcs.d_tiles.as<uint3>() + at;
+            FB_TRY(launch_tile_nl(ctx, nl, P, (uint32_t)v.size(), st));
+            at += v.size();
+        }
+        return FAMSA_OK;
+    }
+};
+
 // Rows [row_begin, row_end) of the packed triangle.  With `bounds` (n_blocks + 1 ascending row indices spanning the
 // range) the work is issued block by block and block_events[b] is recorded after block b, so that a caller can
 // start copying finished blocks while later ones are still being computed; every tile list is uploaded up front.
@@ -708,27 +744,15 @@ int lcs_triangle(famsa_ctx* ctx, uint32_t row_begin, uint32_t row_end, void* d_o
     const uint32_t whole[2] = {row_begin, row_end};
     if (!bounds || !S.identity_perm) { bounds = whole; n_blocks = 1; }
 
-    // tiles per (block, limb-count class); one upload for all of them
-    std::vector<std::vector<std::vector<uint3>>> tiles(n_blocks, std::vector<std::vector<uint3>>(kMaxNL + 1));
-    size_t total = 0;
+    TilePlan tiles(n_blocks);
     for (int b = 0; b < n_blocks; ++b)
         for (uint32_t g = 0; g < S.n_groups; ++g) {
-            const uint32_t nl = S.groups[g].nl;
-            if (nl == 0) continue;
+            if (S.groups[g].nl == 0) continue;
             if (S.identity_perm && (g * 32 + 32 <= bounds[b] || g * 32 >= bounds[b + 1])) continue;
-            const uint32_t q_end = std::min(n, g * 32 + 31);
-            for (uint32_t q0 = 0; q0 < q_end; q0 += kTileQ) {
-                tiles[b][nl].push_back(make_uint3(g, q0, std::min(q_end, q0 + (uint32_t)kTileQ)));
-                ++total;
-            }
+            tiles.add(b, g, S.groups[g].nl, std::min(n, g * 32 + 31));
         }
-    S.last_tiles = total;
-    std::vector<uint3> flat;
-    flat.reserve(total);
-    for (auto& blk : tiles)
-        for (auto& v : blk) flat.insert(flat.end(), v.begin(), v.end());
-    FB_TRY(S.d_tiles.reserve(sizeof(uint3) * std::max<size_t>(total, 1)));
-    if (total) FB_CUDA(cudaMemcpyAsync(S.d_tiles.p, flat.data(), sizeof(uint3) * total, cudaMemcpyHostToDevice, st));
+    S.last_tiles = tiles.total;
+    FB_TRY(tiles.upload(ctx, st));
     TileParams P = base_params(ctx);
     P.out = d_out;
     P.elem_bytes = elem_bytes;
@@ -737,7 +761,6 @@ int lcs_triangle(famsa_ctx* ctx, uint32_t row_begin, uint32_t row_end, void* d_o
     std::vector<uint32_t> special;      // rows the tile kernel may not answer for: dropped-carry and over-long rows
     if (quirk_fixups) std::set_union(S.h_quirky.begin(), S.h_quirky.end(), S.h_long.begin(), S.h_long.end(), std::back_inserter(special));
     else special = S.h_long;         // true LCS everywhere: only the rows the tile kernel cannot reach
-    FB_TRY(mark_tiles_begin(ctx, st));
     // Blocks in one stream would each end with a partly filled last wave (half a wave of tiles per block boundary: 0.4 ms at
     // C2).  Issued round-robin on the auxiliary streams instead, the block scheduler fills the tail of block b with the first
     // tiles of block b+1 and the blocks still finish in order.  (The exact kernels share one scratch: single stream then.)
@@ -747,18 +770,11 @@ int lcs_triangle(famsa_ctx* ctx, uint32_t row_begin, uint32_t row_end, void* d_o
         FB_CUDA(cudaEventRecord(ctx->ev_fork, st));
         for (int a = 0; a < std::min(kAux, n_blocks); ++a) FB_CUDA(cudaStreamWaitEvent(ctx->aux_stream[a], ctx->ev_fork, 0));
     }
-    size_t at = 0;
     for (int b = 0; b < n_blocks; ++b) {
         const cudaStream_t bst = fan ? ctx->aux_stream[b % kAux] : st;
         P.row_begin = bounds[b];
         P.row_end = bounds[b + 1];
-        for (uint32_t nl = 1; nl <= (uint32_t)kMaxNL; ++nl) {
-            auto& v = tiles[b][nl];
-            if (v.empty()) continue;
-            P.tiles = S.d_tiles.as<uint3>() + at;
-            FB_TRY(launch_tile_nl(ctx, nl, P, (uint32_t)v.size(), bst));
-            at += v.size();
-        }
+        FB_TRY(tiles.launch(ctx, b, P, bst));
         // rows the tile kernel cannot answer for: dropped-carry rows entirely; over-long rows only against over-long columns
         // (their pairs with shorter sequences were computed with the shorter one as the mask side -- the true LCS is symmetric)
         std::vector<ExactReq> reqs;
@@ -793,38 +809,18 @@ int lcs_rows(famsa_ctx* ctx, const uint32_t* h_ref_ids, uint32_t n_ref, const ui
     FB_CUDA(cudaMemcpyAsync(S.d_refpos.p, refpos.data(), sizeof(uint32_t) * n_ref, cudaMemcpyHostToDevice, st));
     FB_TRY(S.d_res.reserve((size_t)res_bytes * npad * std::max(1u, n_ref)));
 
-    std::vector<std::vector<uint3>> by_nl(kMaxNL + 1);
+    TilePlan tiles(1);
     g_end = std::min(g_end, S.n_groups);
-    for (uint32_t g = g_begin; g < g_end; ++g) {                     // the mask groups (= columns) this call answers for
-        const uint32_t nl = S.groups[g].nl;
-        if (nl == 0) continue;
-        for (uint32_t q0 = 0; q0 < n_ref; q0 += kTileQ)
-            by_nl[nl].push_back(make_uint3(g, q0, std::min(n_ref, q0 + (uint32_t)kTileQ)));
-    }
-    size_t total = 0;
-    for (auto& v : by_nl) total += v.size();
-    FB_TRY(S.d_tiles.reserve(sizeof(uint3) * std::max<size_t>(total, 1)));
-    size_t at = 0;
-    for (auto& v : by_nl) {
-        if (v.empty()) continue;
-        FB_CUDA(cudaMemcpyAsync(S.d_tiles.as<uint3>() + at, v.data(), sizeof(uint3) * v.size(), cudaMemcpyHostToDevice, st));
-        at += v.size();
-    }
+    for (uint32_t g = g_begin; g < g_end; ++g)                       // the mask groups (= columns) this call answers for
+        if (S.groups[g].nl) tiles.add(0, g, S.groups[g].nl, n_ref);
+    FB_TRY(tiles.upload(ctx, st));
     TileParams P = base_params(ctx);
     P.out = S.d_res.p;
     P.elem_bytes = res_bytes;
     P.rows_mode = 1;
     P.refpos = S.d_refpos.as<uint32_t>();
     P.ld_res = npad;
-    FB_TRY(mark_tiles_begin(ctx, st));
-    at = 0;
-    for (uint32_t nl = 1; nl <= (uint32_t)kMaxNL; ++nl) {
-        auto& v = by_nl[nl];
-        if (v.empty()) continue;
-        P.tiles = S.d_tiles.as<uint3>() + at;
-        FB_TRY(launch_tile_nl(ctx, nl, P, (uint32_t)v.size(), st));
-        at += v.size();
-    }
+    FB_TRY(tiles.launch(ctx, 0, P, st));
     FB_CUDA(cudaEventRecord(ctx->ev[2], st));
     if (n_col && n_ref) {
         dim3 grid((n_col + 255) / 256, n_ref);
@@ -852,29 +848,27 @@ int lcs_rows(famsa_ctx* ctx, const uint32_t* h_ref_ids, uint32_t n_ref, const ui
 // (double) pow(i, 0.75) for every possible indel count into d_pow075_f64, like Transform<double, indel075_div_lcs>'s table
 int lcs_pow075_f64(famsa_ctx* ctx, cudaStream_t st) { return upload_pow075<double>(ctx, ctx->lcs.d_pow075_f64, st); }
 
-// out[k * n_col + i] = LCS with sequence rows[k] as the row (seq0) against col_ids[i], by the reference recurrence for
-// every pair (k_lcs_exact_batch / k_lcs_exact): orientation-exact whatever the two sequences are
-int lcs_exact_block(famsa_ctx* ctx, const std::vector<uint32_t>& rows, const uint32_t* d_col_ids, uint32_t n_col, void* d_out,
-                    int elem_bytes, cudaStream_t st)
-{
-    std::vector<ExactReq> reqs;
-    reqs.reserve(rows.size());
-    for (size_t k = 0; k < rows.size(); ++k) reqs.push_back(ExactReq{rows[k], n_col, 0, k * n_col});
-    return exact_rows(ctx, reqs, d_col_ids, d_out, elem_bytes, st);
-}
-
-// The sequences whose LCS depends on which side is the row (the dropped-carry corner, h_quirky): d_side_idx[caller id] =
-// their row in d_side_rows or -1, and d_side_rows = their n_flagged x n rows (u32) with the flagged sequence as seq0
+// The sequences whose LCS depends on which side is the row (the dropped-carry corner, h_quirky) and every over-long
+// sequence before the last flagged over-long one: lcs_triangle computes a pair of two over-long sequences with the later
+// one as seq0, so the true triangle holds a flagged one's orientation there.  d_side_idx[caller id] = their row in
+// d_side_rows or -1, and d_side_rows = those rows (u32, n wide) with the sequence as seq0 -- what lcs_seq0 reads.
 int lcs_side_rows(famsa_ctx* ctx, cudaStream_t st)
 {
     LcsState& S = ctx->lcs;
-    const uint32_t n = S.n, nq = (uint32_t)S.h_quirky.size();
+    const uint32_t n = S.n;
+    uint32_t long_end = 0;
+    for (uint32_t x : S.h_long)
+        if (std::binary_search(S.h_quirky.begin(), S.h_quirky.end(), x)) long_end = x;
+    std::vector<uint32_t> ids;
+    std::set_union(S.h_quirky.begin(), S.h_quirky.end(), S.h_long.begin(),
+                   std::lower_bound(S.h_long.begin(), S.h_long.end(), long_end), std::back_inserter(ids));
+    const uint32_t nq = (uint32_t)ids.size();
     std::vector<int> side_idx(n, -1);
-    for (uint32_t q = 0; q < nq; ++q) side_idx[S.h_quirky[q]] = (int)q;
+    for (uint32_t q = 0; q < nq; ++q) side_idx[ids[q]] = (int)q;
     FB_TRY(S.d_side_idx.reserve(sizeof(int) * n));
     FB_CUDA(cudaMemcpyAsync(S.d_side_idx.p, side_idx.data(), sizeof(int) * n, cudaMemcpyHostToDevice, st));
     FB_TRY(S.d_side_rows.reserve(std::max<size_t>((size_t)nq * n, 1) * sizeof(uint32_t)));
-    if (nq) FB_TRY(lcs_rows(ctx, S.h_quirky.data(), nq, nullptr, n, S.d_side_rows.p, 4, st));
+    if (nq) FB_TRY(lcs_rows(ctx, ids.data(), nq, nullptr, n, S.d_side_rows.p, 4, st));
     return FAMSA_OK;
 }
 

@@ -166,8 +166,8 @@ struct PrimState {                 // per sequence: best known connection to the
 // against the current vertex (one triangle lookup + one pow-table lookup each, all independent), blocks publish their
 // best (dist, key) pair, ONE grid-wide barrier, and every block reduces the published candidates itself, so all
 // blocks agree on the next vertex without a second barrier.  Candidate slots are double-buffered by step parity.
-// tri: true-LCS triangle in caller order; side rows hold the row-oriented values of the sequences whose LCS is
-// orientation dependent (dropped-carry corner): side_idx[v] = row in `side` or -1.
+// Lookups go through lcs_seq0 on the true-LCS triangle and the side rows (lcs_side_rows), the representation the square
+// distance export reads too.
 // kSlink (famsa_lcs_slink): tri is the triangle SLINK reads (row = seq0, dropped-carry rows exact), every lookup reads
 // it (side_idx and side are not read), and there is no lower-bound skip -- SingleLinkage has none.
 template <bool kSlink>
@@ -200,22 +200,19 @@ __global__ void __launch_bounds__(1024) k_prim(const void* __restrict__ tri, int
     double d0 = 1.7976931348623157e308;
     unsigned long long k0 = 0;
     uint32_t v = 0;
+    const Seq0View L{tri, eb, n, side_idx, side};
     grid.sync();
     for (uint32_t step = 1; step < n; ++step) {
         const uint32_t lv = lens[v];
-        const int sv = kSlink ? -1 : side_idx[v];
+        const int sv = side_row<!kSlink>(L, v);
         PrimCand b = none;
-        auto lookup = [&](uint32_t j) -> uint32_t {
-            if (sv >= 0) return side[(size_t)sv * n + j];
-            return lcs_load(tri, eb, tri_index(v > j ? v : j, v > j ? j : v));
-        };
         // MSTPrim.cpp:450-467: a candidate is only computed when the distance it would have with LCS = the shorter length
         // does not exceed its current one.  A no-op for a true LCS (<= the shorter length); with the dropped-carry corner the
         // reference's LCS can be larger, and then the skip decides whether the candidate is relaxed.
         if (has0 && !vis0) {
             const uint32_t j = gtid;
             const bool tried = kSlink || transform_f64(kind, lv < len0 ? lv : len0, lv, len0, pow075) <= d0;
-            const double d = tried ? transform_f64(kind, lookup(j), lv, len0, pow075) : 1.7976931348623157e308;
+            const double d = tried ? transform_f64(kind, lcs_seq0(L, sv, v, j), lv, len0, pow075) : 1.7976931348623157e308;
             if (tried && d <= d0) {
                 const unsigned long long k = edge_key(v, j);
                 if (d < d0 || k < k0) { d0 = d; k0 = k; }                                  // pair <, given d <= d0
@@ -228,7 +225,7 @@ __global__ void __launch_bounds__(1024) k_prim(const void* __restrict__ tri, int
             unsigned long long ck = st[j].key;
             const uint32_t lj = lens[j];
             const bool tried = kSlink || transform_f64(kind, lv < lj ? lv : lj, lv, lj, pow075) <= cd;
-            const double d = tried ? transform_f64(kind, lookup(j), lv, lj, pow075) : 1.7976931348623157e308;
+            const double d = tried ? transform_f64(kind, lcs_seq0(L, sv, v, j), lv, lj, pow075) : 1.7976931348623157e308;
             if (tried && d <= cd) {
                 const unsigned long long k = edge_key(v, j);
                 if (d < cd || k < ck) { cd = d; ck = k; st[j].dist = cd; st[j].key = ck; }

@@ -1,5 +1,5 @@
 // The packed LCS triangle and the distances read from it: element (hi, lo), hi > lo, of a triangle of u16 or u32 LCS
-// values, and Transform<T, Distance> (reference src/tree/AbstractTreeGenerator.hpp:28-82).  Shared by lcs.cu, tree.cu,
+// values, the LCS with a given sequence as seq0, and Transform<T, Distance> (reference src/tree/AbstractTreeGenerator.hpp:28-82).  Shared by lcs.cu, tree.cu,
 // dist_export.cu and capi.cu.
 #pragma once
 #include <cstddef>
@@ -19,6 +19,31 @@ __host__ __device__ __forceinline__ void lcs_store(void* p, int eb, size_t at, u
 {
     if (eb == 2) static_cast<uint16_t*>(p)[at] = (uint16_t)v;
     else static_cast<uint32_t*>(p)[at] = v;
+}
+
+// The LCS values as the reference computes them, with the row sequence as seq0: the true-LCS triangle (lcs_triangle
+// without quirk fix-ups) and the own rows of the sequences whose value depends on being seq0 (lcs_side_rows).
+struct Seq0View {
+    const void* tri;               // true-LCS triangle, caller order
+    int eb;                        // its element bytes
+    uint32_t n;
+    const int* side_idx;           // caller id -> its row in `side`, or -1
+    const uint32_t* side;          // those rows, n wide, u32
+};
+
+// r's row in `side`, or -1 (always, with kSide = false: no side rows, every lookup reads the triangle).  Read once per
+// row sequence: k_prim issues it at the top of a step, where its latency hides behind the step's other loads.
+template <bool kSide>
+__device__ __forceinline__ int side_row(const Seq0View& L, uint32_t r)
+{
+    return kSide ? L.side_idx[r] : -1;
+}
+
+// LCS with r as seq0 against c, s = side_row(L, r) (r != c, or r has a side row)
+__device__ __forceinline__ uint32_t lcs_seq0(const Seq0View& L, int s, uint32_t r, uint32_t c)
+{
+    if (s >= 0) return L.side[(size_t)s * L.n + c];
+    return lcs_load(L.tri, L.eb, tri_index(r > c ? r : c, r > c ? c : r));
 }
 
 // Transform's distance for "no common residue": (float) nextafter((double) FLT_MAX, 0) == FLT_MAX, and

@@ -65,6 +65,13 @@ def sets():
     out["duplicates"] = base + base[:5] + [base[0]] * 3
     for n in (1, 2, 31, 33, 200):
         out[f"n{n}"] = random_set(rng, n, 1, 500)
+    # flagged sequences before and after unflagged ones, and two over-long sequences whose LCS depends on which one is
+    # seq0, the flagged one second
+    rng = np.random.default_rng(13)
+    long_pair = random_set(rng, 2, 2100, 2400, alphabet=4)
+    long_pair[1][128:192] = 1
+    out["quirk_order"] = (quirk[:2] + random_set(rng, 4, 1, 300) + long_pair[:1] + quirk[2:5] + random_set(rng, 4, 1, 300)
+                          + long_pair[1:] + quirk[5:8])
     return out
 
 

@@ -425,6 +425,20 @@ def test_gpu_prim_edges_match_restatement(engine, monkeypatch, sequential):
             assert np.array_equal(g, w)
 
 
+def test_gpu_prim_over_long_flagged_pair(engine):
+    """Two over-long sequences whose LCS depends on which one is seq0, the flagged one second: the exact path computes
+    their triangle cell with the flagged one as seq0, so Prim's lookup from the first one must read its own side row."""
+    rng = np.random.default_rng(13)
+    cl = random_set(rng, 2, 2100, 2400, alphabet=4)
+    cl[1][128:192] = 1
+    cl += random_set(rng, 6, 60, 260, alphabet=4)
+    codes, offsets, lens = seqio.pack(cl)
+    engine.upload(codes, offsets, lens)
+    for kind in (0, 1):
+        for g, w in zip(engine.prim(kind), _prim_restated(codes, offsets, lens, kind)):
+            assert np.array_equal(g, w)
+
+
 @pytest.mark.parametrize("sequential", [False, True])
 def test_gpu_prim_golden_sl_tree(engine, monkeypatch, sequential):
     """The reference's default guide tree golden (test/adeno_fiber/sl.dnd) without oracle/_ref: the fixture's MST edges
