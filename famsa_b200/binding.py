@@ -18,7 +18,7 @@ EXPORTED_SYMBOLS = [
     "famsa_lcs_last_timing", "famsa_dp_align_batch", "famsa_dp_align_batch_device", "famsa_dp_last_timing",
     "famsa_prof_set_scoring", "famsa_prof_put", "famsa_prof_merge_batch", "famsa_prof_get", "famsa_prof_drop",
     "famsa_prof_last_timing", "famsa_prof_stats", "famsa_prof_align_tree", "famsa_prof_tree_paths",
-    "famsa_prof_refine", "famsa_prof_refined_rows", "famsa_prof_put_rows",
+    "famsa_prof_refine", "famsa_prof_refined_rows", "famsa_prof_put_rows", "famsa_prof_tree_rows",
 ]
 
 PROF_LEAF = 0x80000000            # FAMSA_PROF_LEAF
@@ -57,6 +57,7 @@ class RefineStats(C.Structure):
 
 REFINE_NO_GAP_OPT = 1        # -dgo
 REFINE_NO_TOTAL_SCORE = 2    # -dsp
+REFINE_TREE_ROWS = 4         # famsa_prof_refine on the rows famsa_prof_tree_rows kept on the device
 PUT_ROWS_FROM_TEXT = 1       # famsa_prof_put_rows: the profile the reference builds from rows read as text
 
 
@@ -130,6 +131,7 @@ def load_library() -> C.CDLL:
     lib.famsa_prof_stats.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
     lib.famsa_prof_align_tree.argtypes = [vp, vp, u32, vp, vp, C.POINTER(u32), C.POINTER(u64), vp]
     lib.famsa_prof_tree_paths.argtypes = [vp, vp, u64]
+    lib.famsa_prof_tree_rows.argtypes = [vp, vp, u32, vp, u64, C.POINTER(u32)]
     lib.famsa_prof_refine.argtypes = [vp, u32, vp, u32, u32, vp, u32, C.c_int, C.POINTER(u32), C.POINTER(u32),
                                       C.POINTER(C.c_int64), vp]
     lib.famsa_prof_refined_rows.argtypes = [vp, vp, u64]
@@ -189,6 +191,7 @@ class Engine:
         lens = np.ascontiguousarray(lens, dtype=np.uint32)
         self._check(self.lib.famsa_lcs_upload(self.h, _ptr(codes), _ptr(offsets), _ptr(lens), len(lens)))
         self.n = len(lens)
+        self._tree_width = None
 
     def upload_sorted(self, codes: np.ndarray, offsets: np.ndarray, lens: np.ndarray) -> np.ndarray:
         """famsa_lcs_upload_sorted: indices of later calls are positions in the length-descending order; returns
@@ -198,6 +201,7 @@ class Engine:
         lens = np.ascontiguousarray(lens, dtype=np.uint32)
         self._check(self.lib.famsa_lcs_upload_sorted(self.h, _ptr(codes), _ptr(offsets), _ptr(lens), len(lens)))
         self.n = len(lens)
+        self._tree_width = None
         order = np.zeros(max(self.n, 1), dtype=np.uint32)
         self._check(self.lib.famsa_lcs_sorted_order(self.h, _ptr(order)))
         return order[:self.n]
@@ -505,9 +509,11 @@ class Engine:
         res = (DpResult * max(n, 1))()
         root, nbytes = C.c_uint32(), C.c_uint64()
         st = TreeStats()
+        self._tree_width = None                                     # the kept tree is replaced, or gone if the call fails
         self._check(self.lib.famsa_prof_align_tree(self.h, _ptr(t), n + 1, _ptr(g), C.byref(res), C.byref(root), C.byref(nbytes),
                                                    C.byref(st)))
         stats = {f: getattr(st, f) for f, _ in TreeStats._fields_ if f != "pad"}
+        self._tree_width = int(res[n - 1].path_len)
         out = []
         if want_paths:
             path = np.zeros(max(nbytes.value, 1), dtype=np.uint8)
@@ -529,7 +535,9 @@ class Engine:
         root = C.c_uint32()
         g = np.ascontiguousarray(gaps, dtype=np.int64)
         st = TreeStats()
+        self._tree_width = None
         self._check(self.lib.famsa_prof_align_tree(self.h, _ptr(t), n + 1, _ptr(g), C.byref(res), C.byref(root), C.byref(nbytes), C.byref(st)))
+        self._tree_width = int(res[n - 1].path_len)
         self.prof_drop([root.value])
         return dict(tree=t, n=n, gaps=g, res=res, path=np.zeros(max(int(nbytes.value) * 2, 1), dtype=np.uint8))
 
@@ -537,25 +545,61 @@ class Engine:
         """The two C calls on prebuilt buffers, without this binding's per-merge Python objects.  Returns (root id, stats)."""
         root, nbytes = C.c_uint32(), C.c_uint64()
         st = TreeStats()
+        self._tree_width = None
         self._check(self.lib.famsa_prof_align_tree(self.h, _ptr(b["tree"]), b["n"] + 1, _ptr(b["gaps"]), C.byref(b["res"]), C.byref(root),
                                                    C.byref(nbytes), C.byref(st)))
+        self._tree_width = int(b["res"][b["n"] - 1].path_len)
         self._check(self.lib.famsa_prof_tree_paths(self.h, _ptr(b["path"]), b["path"].size))
         return root.value, {f: getattr(st, f) for f, _ in TreeStats._fields_ if f != "pad"}
 
-    def refine(self, root_id: int, rows, gaps, n_refinements: int = 100, flags: int = 0):
+    def tree_rows(self, order=None, download: bool = True):
+        """famsa_prof_tree_rows: the final alignment of the last align_tree, built on the device -- (n, W) uint8 codes with
+        GAP = 30, row k = leaf order[k] (order None: leaf k).  The rows stay on the device for refine(root, rows=None);
+        download=False leaves them there only and returns None."""
+        o = None if order is None else np.ascontiguousarray(order, dtype=np.uint32)
+        n = self.n if o is None else len(o)
+        w = C.c_uint32()
+        if not download:
+            self._check(self.lib.famsa_prof_tree_rows(self.h, _ptr(o), n, None, 0, C.byref(w)))
+            self._tree_rows_shape = (n, w.value)
+            return None
+        width = getattr(self, "_tree_width", None)
+        if width is not None:               # W_root of the tree align_tree ran
+            out = np.zeros((n, width), dtype=np.uint8)
+            rc = self.lib.famsa_prof_tree_rows(self.h, _ptr(o), n, _ptr(out), out.size, C.byref(w))
+            if rc == 0 and w.value == width:
+                self._tree_rows_shape = (n, width)
+                return out
+        # a tree this binding did not run (or one run behind its back): one device-only call to learn W_root
+        self._check(self.lib.famsa_prof_tree_rows(self.h, _ptr(o), n, None, 0, C.byref(w)))
+        self._tree_width = width = w.value
+        out = np.zeros((n, width), dtype=np.uint8)
+        self._check(self.lib.famsa_prof_tree_rows(self.h, _ptr(o), n, _ptr(out), out.size, C.byref(w)))
+        self._tree_rows_shape = (n, w.value)
+        return out
+
+    def refine(self, root_id: int, rows=None, gaps=None, n_refinements: int = 100, flags: int = 0):
         """famsa_prof_refine: RefineAlignment of the resident root (consumed) whose alignment is `rows` (n x width codes,
-        GAP = 30, rows sorted by FASTA id).  Returns (refined rows, width, total score, stats dict, refined profile id);
-        stats also holds `kernel_launches`, the launches of the call."""
-        r = np.ascontiguousarray(rows, dtype=np.uint8)
+        GAP = 30, rows sorted by FASTA id); rows None: the rows the last tree_rows() kept on the device (FAMSA_REFINE_TREE_ROWS,
+        built in id order).  Returns (refined rows, width, total score, stats dict, refined profile id); stats also holds
+        `kernel_launches`, the launches of the call."""
+        if gaps is None:
+            raise ValueError("gaps are required")
         g = np.ascontiguousarray(gaps, dtype=np.int64)
+        if rows is None:
+            r, (n_rows, width) = None, getattr(self, "_tree_rows_shape", (0, 0))
+            flags |= REFINE_TREE_ROWS
+        else:
+            r = np.ascontiguousarray(rows, dtype=np.uint8)
+            n_rows, width = r.shape
         rid, w, tot = C.c_uint32(), C.c_uint32(), C.c_int64()
         st = RefineStats()
         l0 = self.kernel_launches()
-        self._check(self.lib.famsa_prof_refine(self.h, root_id, _ptr(r), r.shape[0], r.shape[1], _ptr(g), n_refinements, flags,
+        self._check(self.lib.famsa_prof_refine(self.h, root_id, _ptr(r), n_rows, width, _ptr(g), n_refinements, flags,
                                                C.byref(rid), C.byref(w), C.byref(tot), C.byref(st)))
         stats = {f: getattr(st, f) for f, _ in RefineStats._fields_}
         stats["kernel_launches"] = self.kernel_launches() - l0
-        out = np.zeros((r.shape[0], w.value), dtype=np.uint8)
+        out = np.zeros((n_rows, w.value), dtype=np.uint8)
         self._check(self.lib.famsa_prof_refined_rows(self.h, _ptr(out), out.size))
         return out, w.value, tot.value, stats, rid.value
 

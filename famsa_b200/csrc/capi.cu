@@ -235,6 +235,7 @@ int famsa_lcs_upload(famsa_ctx* ctx, const int8_t* codes, const uint64_t* offset
         FB_CUDA(cudaStreamSynchronize(st));                             // earlier *_device calls may still read the old set
         fb::scratch_release(ctx, st, true);
         ctx->lcs.h_order.clear();
+        fb::tree_state_invalidate(ctx);                                 // the leaves of the kept tree change
         return fb::lcs_upload(ctx, codes, offsets, lens, n_seqs);
     });
 }
@@ -702,9 +703,16 @@ int famsa_prof_align_tree(famsa_ctx* ctx, const int32_t* tree, uint32_t n_leaves
                           famsa_dp_result* results, uint32_t* root_id_out, uint64_t* path_bytes_out, famsa_tree_stats* stats)
 {
     return entry(ctx, nullptr, nullptr, [&]() -> int {
+        ctx->prof.tree_valid = false;                                   // a failed call leaves no tree for famsa_prof_tree_rows
         if (!tree || !gaps || !results) { set_error("NULL argument"); return FAMSA_E_INVALID; }
         return FAMSA_OK;
     }, [&](cudaStream_t) { return fb::prof_align_tree(ctx, tree, n_leaves, gaps, results, root_id_out, path_bytes_out, stats); });
+}
+
+int famsa_prof_tree_rows(famsa_ctx* ctx, const uint32_t* order, uint32_t n_rows, uint8_t* rows, uint64_t cap, uint32_t* width_out)
+{
+    return entry(ctx, nullptr, nullptr, [&]() -> int { return FAMSA_OK; },
+                 [&](cudaStream_t) { return fb::prof_tree_rows(ctx, order, n_rows, rows, cap, width_out); });
 }
 
 int famsa_prof_tree_paths(famsa_ctx* ctx, uint8_t* path_buf, uint64_t path_cap)
@@ -720,8 +728,11 @@ int famsa_prof_refine(famsa_ctx* ctx, uint32_t root_id, const uint8_t* rows, uin
                       int64_t* total_score_out, famsa_refine_stats* stats)
 {
     return entry(ctx, nullptr, nullptr, [&]() -> int {
-        if (!rows || !gaps || !refined_id_out || !width_out || !total_score_out) { set_error("NULL argument"); return FAMSA_E_INVALID; }
-        if (flags & ~(FAMSA_REFINE_NO_GAP_OPT | FAMSA_REFINE_NO_TOTAL_SCORE)) { set_error("famsa_prof_refine: unknown flags"); return FAMSA_E_INVALID; }
+        if (flags & FAMSA_REFINE_TREE_ROWS) {
+            if (rows) { set_error("famsa_prof_refine: FAMSA_REFINE_TREE_ROWS takes the kept rows; rows must be NULL"); return FAMSA_E_INVALID; }
+        } else if (!rows) { set_error("NULL argument"); return FAMSA_E_INVALID; }
+        if (!gaps || !refined_id_out || !width_out || !total_score_out) { set_error("NULL argument"); return FAMSA_E_INVALID; }
+        if (flags & ~(FAMSA_REFINE_NO_GAP_OPT | FAMSA_REFINE_NO_TOTAL_SCORE | FAMSA_REFINE_TREE_ROWS)) { set_error("famsa_prof_refine: unknown flags"); return FAMSA_E_INVALID; }
         return FAMSA_OK;
     }, [&](cudaStream_t) {
         return fb::prof_refine(ctx, root_id, rows, n_rows, width, gaps, n_refinements, flags, refined_id_out, width_out, total_score_out, stats);

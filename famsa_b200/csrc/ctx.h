@@ -212,6 +212,17 @@ struct ProfState {
     // result of the most recent famsa_prof_align_tree (pinned): per-merge records and all paths
     famsa_dp_result* h_tree_results = nullptr; size_t h_tree_results_cap = 0;
     uint8_t* h_tree_paths = nullptr; size_t h_tree_paths_cap = 0; uint64_t tree_path_bytes = 0; uint32_t tree_merges = 0;
+    // what famsa_prof_tree_rows needs of the most recent successful famsa_prof_align_tree: its tree, its records in merge
+    // order (path offsets into h_tree_paths) and its root.  tree_valid drops with a failed tree call or a new upload.
+    std::vector<int32_t> tree_kept;
+    std::vector<famsa_dp_result> tree_res;
+    uint32_t tree_root = 0, tree_root_gen = 0;
+    bool tree_valid = false;
+    // the rows of the most recent famsa_prof_tree_rows (row-major, row k = leaf order[k]), for FAMSA_REFINE_TREE_ROWS
+    DevBuf d_tree_rows;
+    uint32_t tree_rows_n = 0, tree_rows_w = 0, tree_rows_root = 0, tree_rows_root_gen = 0;
+    bool tree_rows_valid = false;
+    int tree_rows_occupancy = 0;   // resident k_tree_rows blocks per SM on this context's device (0: not asked yet)
     cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
     cudaEvent_t ev_tree[2] = {nullptr, nullptr};
     uint64_t resident_bytes = 0, n_live = 0;
@@ -323,6 +334,9 @@ int prof_align_tree(famsa_ctx* ctx, const int32_t* tree, uint32_t n_leaves, cons
                     uint32_t* root_id, uint64_t* path_bytes, famsa_tree_stats* stats);
 int prof_tree_paths(famsa_ctx* ctx, uint8_t* path_buf, uint64_t cap);
 void prof_release_all(famsa_ctx* ctx);
+// tree_rows.cu
+int prof_tree_rows(famsa_ctx* ctx, const uint32_t* order, uint32_t n_rows, uint8_t* rows, uint64_t cap, uint32_t* width_out);
+void tree_state_invalidate(famsa_ctx* ctx);      // a new sequence set: the kept tree and rows describe the old one
 // refine.cu
 int prof_refine(famsa_ctx* ctx, uint32_t root_id, const uint8_t* rows, uint32_t n_rows, uint32_t width, const int64_t gaps[4],
                 uint32_t n_refinements, int flags, uint32_t* refined_id, uint32_t* width_out, int64_t* total_score,

@@ -819,6 +819,7 @@ int prof_align_tree(famsa_ctx* ctx, const int32_t* tree, uint32_t n_leaves, cons
 {
     ProfState& P = ctx->prof;
     LcsState& L = ctx->lcs;
+    P.tree_valid = false;                                           // kept only by a call that succeeds
     FB_TRY(ensure_pool(ctx));
     const auto t_begin = std::chrono::steady_clock::now();
     if (n_leaves != L.n) { set_error("famsa_prof_align_tree: the tree has " + std::to_string(n_leaves) + " leaves, " + std::to_string(L.n) + " sequences are uploaded"); return FAMSA_E_INVALID; }
@@ -851,6 +852,12 @@ int prof_align_tree(famsa_ctx* ctx, const int32_t* tree, uint32_t n_leaves, cons
     FB_CUDA(cudaEventElapsedTime(&dev_ms, P.ev_tree[0], P.ev_tree[1]));
     P.tree_path_bytes = R.path_cursor;
     P.tree_merges = n_merges;
+    // for famsa_prof_tree_rows: the tree, the records in merge order and the root
+    P.tree_kept.assign(tree, tree + 2 * (size_t)n_merges);
+    P.tree_res.assign(results, results + n_merges);
+    P.tree_root = R.merged[n_merges - 1];
+    P.tree_root_gen = P.entries[P.tree_root].gen;
+    P.tree_valid = true;
     if (root_id) *root_id = R.merged[n_merges - 1];
     if (path_bytes) *path_bytes = R.path_cursor;
     if (stats) {
@@ -919,6 +926,7 @@ void prof_release_all(famsa_ctx* ctx)
     if (P.h_done) cudaFreeHost(const_cast<unsigned long long*>(P.h_done));
     P.d_block_counter.release();
     P.d_ring_mem.release();
+    P.d_tree_rows.release();
     if (P.h_tree_results) cudaFreeHost(P.h_tree_results);
     if (P.h_tree_paths) cudaFreeHost(P.h_tree_paths);
     for (auto& e : P.ev)

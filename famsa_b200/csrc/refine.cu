@@ -578,7 +578,18 @@ static int refine_run(famsa_ctx* ctx, uint32_t root_id, const uint8_t* rows, uin
                   std::to_string(root_id) + " (" + std::to_string(root.card) + " x " + std::to_string(root.width) + ")");
         return FAMSA_E_INVALID;
     }
-    for (uint32_t r = 0; r < n; ++r) {
+    const bool tree_rows = flags & FAMSA_REFINE_TREE_ROWS;           // the rows famsa_prof_tree_rows kept on the device
+    if (tree_rows && (!P.tree_rows_valid || root_id != P.tree_rows_root || root.gen != P.tree_rows_root_gen || n != P.tree_rows_n ||
+                      width != P.tree_rows_w)) {
+        set_error(P.tree_rows_valid ? "famsa_prof_refine: FAMSA_REFINE_TREE_ROWS: the kept rows (" + std::to_string(P.tree_rows_n) + " x " +
+                                          std::to_string(P.tree_rows_w) + ") belong to root " + std::to_string(P.tree_rows_root) +
+                                          ", not to this root_id / n_rows / width"
+                                    : std::string("famsa_prof_refine: FAMSA_REFINE_TREE_ROWS without rows kept by famsa_prof_tree_rows"));
+        return FAMSA_E_INVALID;
+    }
+    // The kept rows need no check: k_tree_rows writes codes 0..23 and GAP only, and every row holds its sequence's residues,
+    // which is at least one, since famsa_prof_align_tree rejects an empty leaf (prof_resolve) before it keeps a tree.
+    for (uint32_t r = 0; r < n && !tree_rows; ++r) {
         bool residue = false;
         for (uint32_t c = 0; c < width; ++c) {
             const uint8_t v = rows[(size_t)r * width + c];
@@ -608,11 +619,15 @@ static int refine_run(famsa_ctx* ctx, uint32_t root_id, const uint8_t* rows, uin
         if (!e) FB_CUDA(cudaEventCreate(&e));
     cudaEvent_t ev0 = R.ev[0], ev1 = R.ev[1];
     FB_CUDA(cudaEventRecord(ev0, st));
-    // the caller's rows, column-major
+    // the caller's rows (or the kept tree rows), column-major
     {
-        FB_TRY(R.d_cand.reserve((size_t)n * width));
-        FB_CUDA(cudaMemcpyAsync(R.d_cand.p, rows, (size_t)n * width, cudaMemcpyHostToDevice, st));
-        k_ref_transpose<<<dim3(blocks(width, 32), blocks(n, 32)), dim3(32, 8), 0, st>>>(R.d_cand.as<uint8_t>(), R.d_cur.as<uint8_t>(), n, width);
+        const uint8_t* src = P.d_tree_rows.as<uint8_t>();
+        if (!tree_rows) {
+            FB_TRY(R.d_cand.reserve((size_t)n * width));
+            FB_CUDA(cudaMemcpyAsync(R.d_cand.p, rows, (size_t)n * width, cudaMemcpyHostToDevice, st));
+            src = R.d_cand.as<uint8_t>();
+        }
+        k_ref_transpose<<<dim3(blocks(width, 32), blocks(n, 32)), dim3(32, 8), 0, st>>>(src, R.d_cur.as<uint8_t>(), n, width);
         FB_CUDA(cudaGetLastError());
         ++ctx->launches;
     }

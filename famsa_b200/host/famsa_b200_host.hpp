@@ -281,6 +281,24 @@ inline TreeAlignment AlignTree(Context& ctx, const std::vector<std::pair<int, in
     return out;
 }
 
+// The finished alignment of `tree` (the most recent AlignTree on ctx), built on the device by famsa_prof_tree_rows: what
+// FinalizeGaps does at every merge (profile.cpp:1053-1104), with no host work per merge.  Row k is leaf order[k] (empty
+// order: leaf k), width codes each, GAP = 30; a drop-in rebuilds its CGappedSequences from them (INTEGRATION.md).  The rows
+// also stay on the device for famsa_prof_refine with FAMSA_REFINE_TREE_ROWS (order = the id order there).
+struct TreeRowsOut {
+    std::vector<uint8_t> rows;         // n_rows x width, row-major
+    uint32_t n_rows = 0, width = 0;
+};
+inline TreeRowsOut TreeRows(Context& ctx, const TreeAlignment& tree, const std::vector<uint32_t>& order = {})
+{
+    TreeRowsOut out;
+    out.n_rows = (uint32_t)tree.merges.size() + 1;
+    const uint32_t width = tree.merges.empty() ? 0 : (uint32_t)tree.merges.back().path.size();
+    out.rows.resize((size_t)out.n_rows * width);
+    check(famsa_prof_tree_rows(ctx.get(), order.empty() ? nullptr : order.data(), out.n_rows, out.rows.data(), out.rows.size(), &out.width));
+    return out;
+}
+
 // CFAMSA::alignProfiles (msa.cpp:675-718) without its RefineAlignment: the two alignments' profiles as the reference builds
 // them from rows read as text (famsa_prof_put_rows with FAMSA_PUT_ROWS_FROM_TEXT: each profile leaves out its last column)
 // and one unbanded merge.  rows: codes 0..23 or GAP = 30, every row of an alignment as long as its first.  Needs

@@ -407,6 +407,21 @@ int famsa_prof_align_tree(famsa_ctx* ctx, const int32_t* tree, uint32_t n_leaves
                           famsa_tree_stats* stats /* may be NULL */);
 int famsa_prof_tree_paths(famsa_ctx* ctx, uint8_t* path_buf, uint64_t path_cap);
 
+/* The final alignment of the most recent famsa_prof_align_tree: FinalizeGaps of every merge (profile.cpp:1053-1104),
+ * built on the device and kept there.  Row k is leaf order[k] (order NULL: row k = leaf k), W_root codes, GAP = 30.
+ * rows may be NULL (keep on the device only); otherwise n_rows x W_root bytes, row-major, are copied to it (cap bytes).
+ * Each merge's H steps are gap columns in the members of the DP's row profile, its V steps in those of the column
+ * profile (famsa_dp_result.swapped says which child is which); the leaves' residues are the codes of the sequences
+ * already uploaded (famsa_lcs_upload, a code outside 0..23 written as 22, as the leaf profiles count it).  Nothing is
+ * uploaded again but the paths, and no host work is done per merge.  *width_out = W_root.
+ * The rows describe the most recent SUCCESSFUL famsa_prof_align_tree; a later famsa_lcs_upload / famsa_lcs_upload_sorted
+ * or a failed famsa_prof_align_tree leaves none: FAMSA_E_STATE.  FAMSA_E_INVALID: n_rows != the tree's leaves, an order
+ * that is not a permutation of 0..n_rows-1, cap < n_rows x W_root with rows != NULL, width_out NULL.  FAMSA_E_NOMEM: an
+ * allocation failed.  After an error nothing of the call's own stays allocated and the context stays usable.
+ * The rows stay on the device for famsa_prof_refine with FAMSA_REFINE_TREE_ROWS, until the next call of this function. */
+int famsa_prof_tree_rows(famsa_ctx* ctx, const uint32_t* order, uint32_t n_rows, uint8_t* rows, uint64_t cap,
+                         uint32_t* width_out);
+
 /* width/card of a resident profile; scores ((width+1)*32 int64) / counters ((width+1)*32 int32) are
  * copied to the host when non-NULL. */
 int famsa_prof_get(famsa_ctx* ctx, uint32_t id, uint32_t* width, uint32_t* card, int64_t* scores, int32_t* counters);
@@ -438,6 +453,11 @@ int famsa_prof_stats(famsa_ctx* ctx, uint64_t* n_live, uint64_t* resident_bytes)
  * resident.  The context stays usable after any error. */
 #define FAMSA_REFINE_NO_GAP_OPT     1   /* -dgo: CParams::enable_gap_optimization = false */
 #define FAMSA_REFINE_NO_TOTAL_SCORE 2   /* -dsp: CParams::enable_total_score_calculation = false */
+/* FAMSA_REFINE_TREE_ROWS: rows must be NULL; the alignment is the one the most recent famsa_prof_tree_rows kept on the
+ * device, in the order given there -- which must be the id order above, the caller's responsibility as it is for rows.
+ * root_id must be that tree's root (still the same resident profile), n_rows and width must be its; anything else,
+ * or no kept rows, is FAMSA_E_INVALID.  The rows never pass through the host. */
+#define FAMSA_REFINE_TREE_ROWS      4
 
 typedef struct {
     double wall_ms, device_ms;    /* host wall clock of the call; first to last operation on the stream */
