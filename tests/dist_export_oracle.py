@@ -84,6 +84,16 @@ def lcs_square(codes, offsets, lens) -> np.ndarray:
     return pyoracle.lcs_rows(codes, offsets, lens, list(range(n)), n_col=n).astype(np.int64)
 
 
+def expected(code_list, ids, kind: int, square: bool, pid: bool, live: bool = True) -> bytes:
+    """The export of (code_list, ids): the reference's DistanceCalculator where oracle/_ref is built and `live`, else
+    the restatement."""
+    from famsa_b200 import seqio
+    if live and pyoracle.have("ref_dist"):
+        return ref_dist_export([seqio.decode(s) for s in code_list], ids, kind, square, pid, n_threads=8)
+    codes, offsets, lens = seqio.pack(code_list)
+    return csv_from_lcs(lcs_square(codes, offsets, lens), lens, ids, kind, square, pid)
+
+
 # ---------------------------------------------------------------- the reference itself (oracle/_ref, where built)
 def ref_num2str(values) -> list[bytes]:
     """The reference's num2str on float32 values (one call for all of them)."""

@@ -13,12 +13,10 @@ from famsa_b200 import seqio
 from famsa_b200.binding import WRITE_FN
 from conftest import GOLDEN, QUIRK_SEQS, random_set
 import dist_export_oracle as O
-from oracle import pyoracle
 from test_dist_export_host import MODES, TABLE, wrapping_floats
 
 pytestmark = pytest.mark.gpu
 
-LETTERS = "ARNDCQEGHILKMFPSTWYVBZX*"
 E_INVALID, E_STATE, E_SINK = 1, 4, 6
 EXPORT_MODES = [(0, False, False), (1, False, False), (0, False, True), (0, True, False), (1, True, False), (0, True, True)]
 
@@ -40,14 +38,6 @@ def test_adeno_goldens(engine, golden, name, square, pid, chunk_bytes):
     total, main, cells = engine.last_timing()
     n = len(golden["ids"])
     assert cells == (n * n if square else n * (n - 1) // 2) and total >= main > 0
-
-
-def expected(code_list, ids, kind, square, pid):
-    if pyoracle.have("ref_dist"):
-        letters = ["".join(LETTERS[c] for c in s) for s in code_list]
-        return O.ref_dist_export(letters, ids, kind, square, pid, n_threads=8)
-    codes, offsets, lens = seqio.pack(code_list)
-    return O.csv_from_lcs(O.lcs_square(codes, offsets, lens), lens, ids, kind, square, pid)
 
 
 def sets():
@@ -84,7 +74,7 @@ def test_equals_reference(engine, case, kind, square, pid):
     code_list = SETS[case]
     ids = [f"{case}_{i}|x y/{len(c)}" for i, c in enumerate(code_list)]
     engine.upload(*seqio.pack(code_list))
-    assert engine.dist_export(ids, kind, square, pid, chunk_bytes=4096) == expected(code_list, ids, kind, square, pid)
+    assert engine.dist_export(ids, kind, square, pid, chunk_bytes=4096) == O.expected(code_list, ids, kind, square, pid)
 
 
 def test_out_file_object(engine, golden):
@@ -120,10 +110,12 @@ def test_device_formatter(engine):
     assert engine.debug_format_f32(np.array([v for v, _ in TABLE], np.float32)) == b"".join(t + b"," for _, t in TABLE)
 
 
-def raw_export(engine, ids, sink, kind=0, square=0, pid=0, chunk=0, id_blob=True):
-    blob = b"".join(i.encode() for i in ids)
-    offs = np.zeros(len(ids) + 1, dtype=np.uint64)
-    offs[1:] = np.cumsum([len(i.encode()) for i in ids])
+def raw_export(engine, ids, sink, kind=0, square=0, pid=0, chunk=0, id_blob=True, prefix=b""):
+    """famsa_dist_export through the C ABI; the id blob starts with `prefix`, which id_offsets[0] skips."""
+    raw = [i.encode() if isinstance(i, str) else bytes(i) for i in ids]
+    blob = prefix + b"".join(raw)
+    offs = np.full(len(raw) + 1, len(prefix), dtype=np.uint64)
+    offs[1:] += np.cumsum([len(i) for i in raw], dtype=np.uint64)
     written = C.c_uint64()
     cb = WRITE_FN(sink)
     rc = engine.lib.famsa_dist_export(engine.h, kind, square, pid, C.c_char_p(blob) if id_blob else None,
